@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """
-bench.py — headline benchmark of the DeTikZify hot path on B200 (contract in the task brief, tier ④).
+bench.py — headline benchmark of the DeTikZify hot path on an H100.
 
 Workload (BASELINE.json configs[1], named in ``config.workload``): detikzify-ds-1.3b shape, random-init
 bf16 weights, ONE synthetic 384x384 figure per GPU, batch-1 greedy generation: ViT encode + concat-3
@@ -27,6 +27,12 @@ quota.
 Multi-GPU: figures are independent -> one engine per rank, ONE NCCL broadcast of the weight arena at
 load, no per-step collective; scaling is weak (one figure per GPU per step); every rank is pinned to the NUMA node of
 its GPU.
+
+``--dump-outputs DIR`` writes what the last timed step computed as ``DIR/<name>.npy`` so that two builds can be compared
+output for output (inputs and weights are seeded, so the same arguments give the same inputs): image embeddings, prefill
+logits, the first token and the last 256 tokens of the device-side loop (what the engine's token ring still holds), the
+token ids ``model.generate()`` returned, the pooled ViT output of every batch size of the sweep, and the last token of every
+ds-7b rollout.
 """
 from __future__ import annotations
 
@@ -62,6 +68,7 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-vit-sweep", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -116,20 +123,7 @@ def peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(kernel: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of ``kernel`` from the committed `ncu --set full` capture
-    (profiles/r*_ncu_full_<kernel>.json, written by tools/ncu_summary.py); None when no capture is committed."""
-    best = None
-    for f in sorted((ROOT / "profiles").glob(f"r*_ncu_full_{kernel}.json")):
-        try:
-            d = json.loads(f.read_text())
-            best = {"bytes_per_launch": d["dram_bytes_read"] + d["dram_bytes_write"], "ctx": d.get("ctx"), "source": f"profiles/{f.name}"}
-        except (OSError, ValueError, KeyError):
-            continue
-    return best
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 # ---------------------------------------------------------------------------------- CPU reference arm
@@ -283,8 +277,9 @@ def run_ours(args):
 
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
 
-    def figure(timed: bool):
-        """ViT -> projector -> prefill -> first token -> (n_new - 1) graph-launched decode+sample steps."""
+    def figure(timed: bool, keep: bool = False):
+        """ViT -> projector -> prefill -> first token -> (n_new - 1) graph-launched decode+sample steps.
+        keep: also read back the steps the token ring still holds (256) and return the step's outputs."""
         if timed:
             ev[0].record(stream)
         img = eng.image_embeds(pix_dev)[0]
@@ -299,8 +294,12 @@ def run_ours(args):
         if timed:
             ev[2].record(stream)
         out = eng.gen_wait(n_new - 2)  # last token has landed on the host
+        kept = None
+        if keep:
+            tail = [eng.gen_wait(i)[0] for i in range(max(0, n_new - 1 - 256), n_new - 1)]
+            kept = {"image_embeds": img, "prefill_logits": last, "loop_first_token": [tok0], "loop_last_tokens": tail}
         eng.gen_end()
-        return out
+        return kept
 
     def barrier():
         torch.cuda.synchronize()
@@ -320,8 +319,9 @@ def run_ours(args):
         start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         start.record(stream)
         dec_ms = []
-        for _ in range(args.steps):
-            figure(True)
+        outputs = {}
+        for i in range(args.steps):
+            outputs = figure(True, keep=bool(args.dump_outputs) and i == args.steps - 1) or outputs
             stream.synchronize()
             dec_ms.append(ev[1].elapsed_time(ev[2]))
         stop.record(stream)
@@ -352,7 +352,7 @@ def run_ours(args):
             for _ in range(args.steps):
                 model._img_cache = None      # a new figure every step: ViT + full prefill inside the timed region
                 model._slot_tokens = []
-                api_figure()
+                outputs["generate_ids"] = api_figure()
             torch.cuda.synchronize()
             e2e_t = time.perf_counter() - t0
             barrier()
@@ -369,12 +369,24 @@ def run_ours(args):
                 reps = 5 if B < 64 else 3
                 v0.record(stream)
                 for _ in range(reps):
-                    eng.vit_encode(pix_b)
+                    _, pooled = eng.vit_encode(pix_b)
                 v1.record(stream)
                 stream.synchronize()
+                outputs[f"vit_pooled_b{B}"] = pooled
                 vit[str(B)] = v0.elapsed_time(v1) / reps / B
                 del pix_b
         barrier()
+
+    def dump(named):   # all together about 2.5 MB as float32 (243 x 2048 embeddings, 32256 logits, 73 x 1152 pooled rows, ids)
+        import numpy as np
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        suffix = f".rank{rank}" if world > 1 else ""
+        for name, t in named.items():
+            np.save(out_dir / f"{name}{suffix}.npy", torch.as_tensor(t).detach().float().cpu().numpy())
+
+    if args.dump_outputs:
+        dump(outputs)
 
     # ---- BASELINE.json configs[3] / configs[4] shape: detikzify-ds-7b, figures striped over the ranks, 32 nucleus-sampled
     # rollouts per figure forked off one prefilled 243-token image prompt. Extra keys; the headline stays configs[1].
@@ -440,6 +452,8 @@ def run_ours(args):
             barrier()
             roll_s = g0.elapsed_time(g1) / 1e3
             launches7 = e7.launch_count - l0
+        if args.dump_outputs:
+            dump({"ds7b_rollout_last_tokens": local_out})   # [figures of this rank, rollouts]
         gathered = gather_results([(g, o[:4]) for g, o in zip(figures, local_out)])   # one gather at the end (examples/eval.py:132)
         t7 = torch.tensor([b1_ms, roll_s, float(len(gathered))], dtype=torch.float64)
         kvb = e7.decode_bytes(1) - e7.decode_bytes(0)
@@ -487,17 +501,16 @@ def run_ours(args):
         achieved = bytes_dec * args.steps / t_dec / 1e9
         kernel_name = ("decode_mega_kernel (persistent cooperative weight-streaming decode kernel, 1 launch per token) + sample_kernel"
                        if persistent else "decode step (CUDA graph: fused RMSNorm+GEMV / split-K attention / sampler kernels of one token)")
-        traffic = ncu_traffic("decode_mega_kernel") if persistent else None
         line = {
             "metric": "TikZ tokens/sec/GPU (decode, 384px cond, 2k ctx)", "value": value, "unit": "tokens/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": t_all / args.steps * 1e3,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": f"{args.model} random-init bf16, 1x384px synthetic figure per GPU, batch-1 greedy: ViT + projector + "
                                    f"{P}-token prefill + {n_new} decoded tokens to total length {total}",
-                       "l2": "inputs larger than L2: 2.56 GB of weights streamed per token (126 MB L2)",
+                       "l2": "inputs larger than L2: 2.56 GB of weights streamed per token (50 MB L2)",
                        "parallelism": f"figure-sharded dp{world}, 1 NCCL weight broadcast at load, no per-step collective"},
             "roofline": {"bound": "hbm", "kernel": kernel_name,
-                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+                         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "bytes_per_token_avg": bytes_dec / (n_new - 1),
                          "decode_ms_per_token": t_dec / args.steps / (n_new - 1) * 1e3},
             "gpu_launches": int(launches),
@@ -509,7 +522,7 @@ def run_ours(args):
             n_tok = (vc.image_size // vc.patch_size) ** 2
             D, Iv, Lv = vc.hidden_size, vc.intermediate_size, vc.num_hidden_layers
             flop_img = Lv * (2 * n_tok * (4 * D * D + 2 * D * Iv) + 4 * n_tok * n_tok * D) + 2 * n_tok * D * 3 * vc.patch_size ** 2
-            tpeak, tsrc = 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)"
+            tpeak, tsrc = 989.0, "fallback (H100 SXM data sheet: 989 TFLOP/s dense bf16)"
             pk = ROOT / "MEASURED_PEAKS.json"
             if pk.exists() and json.loads(pk.read_text()).get("bf16_tflops_sustained"):
                 tpeak, tsrc = float(json.loads(pk.read_text())["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"

@@ -1,5 +1,5 @@
 """
-In-tree build of the C-ABI CUDA library (``detikzify_b200/csrc/libdtk_b200.so``) for sm_100a.
+In-tree build of the C-ABI CUDA library (``detikzify_b200/csrc/libdtk_b200.so``) for sm_90a.
 
 nvcc cross-compiles without a GPU. Each ``.cu`` is compiled to an object in ``csrc/build/`` (parallel,
 re-compiled only when the source or a header is newer) and linked into one shared library that exports
@@ -17,7 +17,7 @@ CSRC = Path(__file__).resolve().parent / "csrc"
 ROOT = Path(__file__).resolve().parent.parent
 LIB = CSRC / "libdtk_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
           "-Xptxas", "-v", "-I", str(ROOT / "include")]
 

@@ -1,91 +1,33 @@
-// tcgen05 flash attention for the ViT (SigLIP so400m: 16 heads x head_dim 72, N = 729 keys, non-causal)
+// wgmma flash attention for the ViT (SigLIP so400m: 16 heads x head_dim 72, N = 729 keys, non-causal)
 //   HF modeling_siglip.py:229-249,293-306 (softmax(q k^T * d^-1/2) v), reference call site v1/modeling_detikzify.py:63-72.
 //
-// One CTA = 128 queries of one (image, head); 192 threads, warp-specialised like gemm_tc.cu:
-//   warp 4  TMA producer : Q once, then per 128-key block K (rank-3 map over the qkv matrix viewed as
-//                          [token][3*heads][72]: the 64..127 half of the padded head_dim lies past extent 72 and is ZERO
-//                          filled by TMA) and V^T (from the per-layer transposed copy, keys contiguous) into a 2-stage ring
-//   warp 5  MMA issuer   : S = Q K^T (M128 x N128 x K80: 5 tcgen05.mma) into TMEM columns [0,128); after the softmax
-//                          warps have written P: PV = P V (M128 x N80 x K128: 8 tcgen05.mma) into TMEM columns [128,208)
-//   warps 0-3 softmax    : thread = query row = TMEM lane. Two passes over S with tcgen05.ld (row max, then exp2 / sum) —
-//                          no shuffles, the whole row lives in one thread — P as bf16 into a SWIZZLE_128B K-major tile
-//                          (manual XOR swizzle, same layout TMA writes), PV read back and folded into the fp32 output
-//                          registers with the online-softmax rescale (the accumulator never needs a TMEM round trip).
+// One CTA = 128 queries of one (image, head); 288 threads, warp-specialised like gemm_tc.cu:
+//   warp 8      TMA producer : Q once, then per 128-key block K (rank-3 map over the qkv matrix viewed as
+//                              [token][3*heads][72]: the 64..127 half of the padded head_dim lies past extent 72 and is
+//                              ZERO filled by TMA) and V^T (from the per-layer transposed copy, keys contiguous) into a
+//                              2-stage ring
+//   warps 0-7   two consumer warpgroups, 64 queries each: S = Q K^T (m64n128, K = 80: 5 wgmma from shared-memory
+//                              descriptors) into registers; online softmax on the accumulator layout (a row lives in the
+//                              four lanes of a quad: two shuffles per reduction); P as bf16 straight into the register
+//                              A operand of PV = P V (m64n80, K = 128: 8 wgmma, B = V^T tile), accumulated on top of the
+//                              rescaled fp32 output registers.
 // Keys past the image's 729 (rows of the next image / zero padding of V^T) are masked to -inf before the softmax.
 // All mbarrier waits are bounded (trap instead of hanging the GPU).
 #include <cuda.h>
 
 #include "common.cuh"
 #include "launch.h"
+#include "wgmma.cuh"
 
 namespace dtk {
 namespace {
 
 constexpr int AQ = 128, AK = 128, DH = 72, DP = 80;       // queries / keys per block, head_dim, padded to the mma K step
-constexpr int ATC_THREADS = 192;
+constexpr int ATC_THREADS = 288;
 constexpr int QB = AQ * 128;                                // one [128 rows x 64 cols] bf16 SWIZZLE_128B block = 16 KB
 constexpr int VB = DP * 128;                                // one [80 rows x 64 keys] block = 10 KB
 constexpr int KV_STAGE = 2 * QB + 2 * VB;                   // K (2 blocks) + V^T (2 blocks)
-constexpr int ATC_SMEM = 2 * QB /*Q*/ + 2 * KV_STAGE + 2 * QB /*P*/ + 1024 + 256;
-constexpr long long ATC_SPIN = 2000000000ll;
-
-DTK_DEV void a_mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count)); }
-DTK_DEV void a_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory"); }
-DTK_DEV void a_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory"); }
-DTK_DEV void a_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  long long t0 = 0;
-  while (!done) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (!done && (++spins & 1023u) == 0) {
-      const long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > ATC_SPIN) __trap();
-    }
-  }
-}
-DTK_DEV void a_tma_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
-               : "memory");
-}
-DTK_DEV void a_tma_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar)
-               : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (see gemm_tc.cu)
-DTK_DEV uint64_t a_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-DTK_DEV void a_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-DTK_DEV void a_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-DTK_DEV void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-DTK_DEV void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
+constexpr int ATC_SMEM = 2 * QB /*Q*/ + 2 * KV_STAGE + 1024 + 256;
 
 struct AttnTcArgs {
   bf16* o;                   // [B*N, D] bf16, head h at columns h*72
@@ -97,170 +39,124 @@ struct AttnTcArgs {
 __global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap mapQK,
                                                                  const __grid_constant__ CUtensorMap mapVT, const AttnTcArgs p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sraw = smem_u32(smem_raw);
-  const uint32_t sbase = (sraw + 1023u) & ~1023u;
-  const uint32_t sQ = sbase, sKV = sQ + 2 * QB, sP = sKV + 2 * KV_STAGE;
-  const uint32_t bars = sP + 2 * QB;
-  // barriers: q_full, kv_full[2], kv_empty[2], s_full, p_full, pv_full, then the TMEM pointer
-  const uint32_t q_full = bars, kv_full0 = bars + 8, kv_empty0 = bars + 24, s_full = bars + 40, p_full = bars + 48, pv_full = bars + 56,
-                 tptr = bars + 64;
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sQ = sbase, sKV = sQ + 2 * QB;
+  const uint32_t bars = sKV + 2 * KV_STAGE;
+  // barriers: q_full, kv_full[2], kv_empty[2]
+  const uint32_t q_full = bars, kv_full0 = bars + 8, kv_empty0 = bars + 24;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * AQ;
   const int nblk = (p.N + AK - 1) / AK;
 
   if (threadIdx.x == 0) {
-    a_mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { a_mbar_init(kv_full0 + 8 * s, 1); a_mbar_init(kv_empty0 + 8 * s, 1); }
-    a_mbar_init(s_full, 1);
-    a_mbar_init(p_full, 128);
-    a_mbar_init(pv_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_init(q_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(kv_full0 + 8 * s, 1); mbar_init(kv_empty0 + 8 * s, 8); }   // empty: one arrive per consumer warp
+    mbar_init_fence();
   }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tptr), "n"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem) : "r"(tptr));
-  const uint32_t tS = tmem, tO = tmem + 128;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ===== TMA producer
     if (lane == 0) {
       const int row0 = b * p.N;
-      a_expect_tx(q_full, 2 * QB);
-      a_tma_3d(sQ, &mapQK, 0, head, row0 + q0, q_full);                 // d 0..63
-      a_tma_3d(sQ + QB, &mapQK, 64, head, row0 + q0, q_full);           // d 64..127 (>= 72: zero fill)
+      mbar_expect_tx(q_full, 2 * QB);
+      tma_load_3d(sQ, &mapQK, 0, head, row0 + q0, q_full);                 // d 0..63
+      tma_load_3d(sQ + QB, &mapQK, 64, head, row0 + q0, q_full);           // d 64..127 (>= 72: zero fill)
       for (int j = 0; j < nblk; ++j) {
         const int s = j & 1, use = j >> 1;
-        if (use > 0) a_wait(kv_empty0 + 8 * s, (use - 1) & 1);
+        if (use > 0) mbar_wait(kv_empty0 + 8 * s, (use - 1) & 1);
         const uint32_t sk = sKV + s * KV_STAGE, sv = sk + 2 * QB;
-        a_expect_tx(kv_full0 + 8 * s, KV_STAGE);
-        a_tma_3d(sk, &mapQK, 0, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
-        a_tma_3d(sk + QB, &mapQK, 64, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
-        a_tma_2d(sv, &mapVT, j * AK, (b * p.heads + head) * DP, kv_full0 + 8 * s);
-        a_tma_2d(sv + VB, &mapVT, j * AK + 64, (b * p.heads + head) * DP, kv_full0 + 8 * s);
+        mbar_expect_tx(kv_full0 + 8 * s, KV_STAGE);
+        tma_load_3d(sk, &mapQK, 0, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
+        tma_load_3d(sk + QB, &mapQK, 64, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
+        tma_load_2d(sv, &mapVT, j * AK, (b * p.heads + head) * DP, kv_full0 + 8 * s);
+        tma_load_2d(sv + VB, &mapVT, j * AK + 64, (b * p.heads + head) * DP, kv_full0 + 8 * s);
       }
     }
-  } else if (warp == 5) {
-    // ===== MMA issuer (instruction descriptor: D=F32, A=B=BF16, both K-major, N>>3 at bit 17, M>>4 at bit 24)
-    const uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AK >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-    const uint32_t idesc_o = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(DP >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-    if (lane == 0) {
-      a_wait(q_full, 0);
-      for (int j = 0; j < nblk; ++j) {
-        const int s = j & 1, use = j >> 1;
-        a_wait(kv_full0 + 8 * s, use & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t sk = sKV + s * KV_STAGE, sv = sk + 2 * QB;
-        // S = Q K^T over head_dim 80 = 4 k-steps of block 0 + 1 k-step of block 1 (the softmax warps have finished
-        // reading the previous S: they arrived on p_full before the previous PV, which this thread waited for)
+    return;
+  }
+  // ===== consumer warpgroup wg: this thread holds query rows q0 + 64 wg + 16 (warp % 4) + g and + 8 (accumulator layout in wgmma.cuh)
+  const int wg = warp >> 2, g = lane >> 2, c = lane & 3;
+  const uint32_t sQw = sQ + wg * (64 * 128);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, o[DP / 2];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) a_mma(tS, a_desc(sQ + k * 32), a_desc(sk + k * 32), idesc_s, k != 0);
-        a_mma(tS, a_desc(sQ + QB), a_desc(sk + QB), idesc_s, 1);
-        a_commit(s_full);
-        // PV = P V over the 128 keys of the block (2 blocks of 4 k-steps)
-        a_wait(p_full, j & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+  for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int s = j & 1, use = j >> 1;
+    mbar_wait(kv_full0 + 8 * s, use & 1);
+    const uint32_t sk = sKV + s * KV_STAGE, sv = sk + 2 * QB;
+    // S = Q K^T over head_dim 80 = 4 k-steps of block 0 + 1 k-step of block 1
+    float sc[AK / 2];
+    wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 8; ++k)
-          a_mma(tO, a_desc(sP + (k >> 2) * QB + (k & 3) * 32), a_desc(sv + (k >> 2) * VB + (k & 3) * 32), idesc_o, k != 0);
-        a_commit(pv_full);
-        a_commit(kv_empty0 + 8 * s);          // K / V^T stage free once these MMAs have read it
-      }
-    }
-  } else {
-    // ===== softmax warps 0..3: thread = query row q0 + 32 w + lane = TMEM lane
-    const int row = warp * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
-    float m_run = -INFINITY, l_run = 0.f, o[DP];
+    for (int k = 0; k < 4; ++k) wgmma_m64n128k16_ss(sc, wgmma_desc(sQw + k * 32), wgmma_desc(sk + k * 32), k != 0);
+    wgmma_m64n128k16_ss(sc, wgmma_desc(sQw + QB), wgmma_desc(sk + QB), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_acc_fence(sc);
+    const int kvalid = min(AK, p.N - j * AK);           // keys of this block that belong to the image
+    float alpha[2], m_new[2];
 #pragma unroll
-    for (int i = 0; i < DP; ++i) o[i] = 0.f;
-    const uint32_t prow = sP + (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u;   // row base inside a 64-col block
-    for (int j = 0; j < nblk; ++j) {
-      a_wait(s_full, j & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      const int kvalid = min(AK, p.N - j * AK);           // keys of this block that belong to the image
-      // pass 1: row maximum
+    for (int h = 0; h < 2; ++h) {   // h = 0: row g, h = 1: row g + 8
       float mx = -INFINITY;
-#pragma unroll 1
-      for (int cb = 0; cb < AK; cb += 32) {
-        uint32_t r[32];
-        tmem_ld32(tS + lane_sel + (uint32_t)cb, r);
 #pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (cb + i < kvalid) mx = fmaxf(mx, __uint_as_float(r[i]));
+      for (int jj = 0; jj < AK / 8; ++jj) {
+        const int col = 8 * jj + 2 * c;
+        if (col < kvalid) mx = fmaxf(mx, sc[4 * jj + 2 * h]);
+        if (col + 1 < kvalid) mx = fmaxf(mx, sc[4 * jj + 2 * h + 1]);
       }
-      const float m_new = fmaxf(m_run, mx * p.scale_log2);
-      const float alpha = exp2f(m_run - m_new);             // first block: exp2(-inf) = 0
-      // pass 2: p = exp2(s * scale - m), row sum, P (bf16) into the swizzled A tile
-      float ps = 0.f;
-#pragma unroll 1
-      for (int cb = 0; cb < AK; cb += 32) {
-        uint32_t r[32];
-        tmem_ld32(tS + lane_sel + (uint32_t)cb, r);
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = (cb + i < kvalid) ? exp2f(__uint_as_float(r[i]) * p.scale_log2 - m_new) : 0.f;
-          const float p1 = (cb + i + 1 < kvalid) ? exp2f(__uint_as_float(r[i + 1]) * p.scale_log2 - m_new) : 0.f;
-          // the denominator uses the bf16-rounded probabilities the tensor core multiplies with
-          const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
-          ps += __low2float(pb) + __high2float(pb);
-          pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&pb);
-        }
-        // 32 keys = 4 chunks of 16 B; key column c -> block c / 64, chunk (c % 64) / 8, XOR-swizzled with the row
-        const uint32_t blk = prow + (uint32_t)(cb >> 6) * QB;
-#pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {
-          const uint32_t chunk = (uint32_t)(((cb & 63) >> 3) + ch) ^ (uint32_t)(row & 7);
-          asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};\n" ::"r"(blk + chunk * 16u), "r"(pk[4 * ch]), "r"(pk[4 * ch + 1]),
-                       "r"(pk[4 * ch + 2]), "r"(pk[4 * ch + 3])
-                       : "memory");
-        }
-      }
-      l_run = l_run * alpha + ps;
-      m_run = m_new;
-      // P is read by the tensor core through the async proxy
-      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      a_arrive(p_full);
-      // fold PV into the output registers
-      a_wait(pv_full, j & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-#pragma unroll
-      for (int cb = 0; cb < DP; cb += 16) {
-        uint32_t r[16];
-        tmem_ld16(tO + lane_sel + (uint32_t)cb, r);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) o[cb + i] = o[cb + i] * alpha + __uint_as_float(r[i]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      m_new[h] = fmaxf(m_run[h], mx * p.scale_log2);
+      alpha[h] = exp2f(m_run[h] - m_new[h]);             // first block: exp2(-inf) = 0
+      m_run[h] = m_new[h];
     }
-    // normalise + store 72 bf16 (144 B, 16-byte aligned) of this row
-    const int q = q0 + row;
+    // p = exp2(s * scale - m) as bf16 in the A-fragment layout of the 8 k-steps (16 keys each) of PV
+    uint32_t pa[AK / 16][4];
+    float ps[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < AK / 8; ++jj) {
+      const int col = 8 * jj + 2 * c;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float p0 = (col < kvalid) ? exp2f(sc[4 * jj + 2 * h] * p.scale_log2 - m_new[h]) : 0.f;
+        const float p1 = (col + 1 < kvalid) ? exp2f(sc[4 * jj + 2 * h + 1] * p.scale_log2 - m_new[h]) : 0.f;
+        // the denominator uses the bf16-rounded probabilities the tensor core multiplies with
+        const __nv_bfloat162 pb = __floats2bfloat162_rn(p0, p1);
+        ps[h] += __low2float(pb) + __high2float(pb);
+        pa[jj >> 1][(jj & 1) * 2 + h] = *reinterpret_cast<const uint32_t*>(&pb);
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + ps[h];   // per-thread partial of the row sum (reduced over the quad at the end)
+#pragma unroll
+    for (int i = 0; i < DP / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+    // O += P V over the 128 keys of the block (2 V^T blocks of 4 k-steps)
+    wgmma_acc_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k) wgmma_m64n80k16_rs(o, pa[k], wgmma_desc(sv + (k >> 2) * VB + (k & 3) * 32), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_acc_fence(o);
+    if (lane == 0) mbar_arrive(kv_empty0 + 8 * s);          // K / V^T stage free once this warp's MMAs have read it
+  }
+  // normalise + store the 72 bf16 of the two rows
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int q = q0 + wg * 64 + (warp & 3) * 16 + g + 8 * h;
     if (q < p.N) {
-      const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
+      const float inv = l > 0.f ? 1.f / l : 0.f;
       bf16* dst = p.o + (int64_t)(b * p.N + q) * p.o_rs + head * DH;
 #pragma unroll
-      for (int c = 0; c < DH; c += 8) {
-        uint4 v;
-        v.x = pack_bf16x2(o[c] * inv, o[c + 1] * inv);
-        v.y = pack_bf16x2(o[c + 2] * inv, o[c + 3] * inv);
-        v.z = pack_bf16x2(o[c + 4] * inv, o[c + 5] * inv);
-        v.w = pack_bf16x2(o[c + 6] * inv, o[c + 7] * inv);
-        *reinterpret_cast<uint4*>(dst + c) = v;
-      }
+      for (int jj = 0; jj < DH / 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj + 2 * c) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
     }
-  }
-  __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(256));
   }
 }
 

@@ -270,7 +270,7 @@ cudaError_t launch_gemv(const GemvArgs& a, cudaStream_t s, uint64_t* counter) {
   const int smem = a.K * (int)sizeof(float);
   const int items = a.N / 2;
   int gx = (items + 7) / 8;
-  if (gx > 296) gx = 296;  // 2 CTAs per SM x 148 SMs; warps loop over the remaining items
+  if (gx > 264) gx = 264;  // 2 CTAs per SM x 132 SMs; warps loop over the remaining items
   dim3 grid(gx, a.B);
   cudaError_t e = cudaSuccess;
 #define DTK_GEMV_CASE(M)                                                                                        \

@@ -2,15 +2,15 @@
 //
 // Why: batch-1 decode streams every decoder weight once per token (2.56 GB for ds-1.3b) through ~120
 // dependent GEMV-sized steps of a few microseconds each. Launched as separate kernels (even from a
-// CUDA graph) the HBM pipe drains at every step boundary and the chain is launch/ramp bound
-// (measured 0.37 of the HBM roofline). Here the weight stream is decoupled from the dependency chain:
+// CUDA graph) the HBM pipe drains at every step boundary and the chain is launch/ramp bound.
+// Here the weight stream is decoupled from the dependency chain:
 //
 //   * grid = one CTA per SM, resident for the whole token (cooperative launch);
 //   * 4 PRODUCER warps per CTA (one issuing lane each, registers handed back with setmaxnreg.dec) walk the
 //     CTA's statically known list of weight tiles AND cached key/value items for ALL layers and phases and stream
 //     them with 1-D TMA bulk copies (cp.async.bulk + mbarrier complete_tx) into a ~190 KB shared-memory ring of
 //     8 KB slots, never waiting for activations — neither weights nor the cache depend on this token — so HBM
-//     stays busy across phase boundaries (the ring alone sustains 7.2 TB/s, profiles/r2_stream_per_sm.txt);
+//     stays busy across phase boundaries;
 //   * 8 CONSUMER warps (setmaxnreg.inc: the kernel calls no function, or ptxas would ignore setmaxnreg) take
 //     tiles in order. A tile is 16 output rows x 256 k, pre-arranged in HBM (launch_retile, once at load) so that
 //     it lands in shared memory exactly in ldmatrix.x4 order; the dot products run on the tensor pipe (mma.sync
@@ -32,7 +32,7 @@
 // Per layer: P1 qkv(+RMSNorm, RoPE, KV write) | P2 split-KV attention (the CTA's share of the cached keys/values
 // arrives through the ring; a fixed owner CTA per head merges the partials) | P3 o-proj + residual | P4 gate/up +
 // SiLU*mul (+RMSNorm) | P5 down + residual; finally lm_head (+final RMSNorm, + greedy argmax and token publication
-// in the kernel tail). DESIGN.md section 4 lists the measured alternatives that were rejected.
+// in the kernel tail). DESIGN.md section 4 describes the design.
 //
 // Replaces the per-token HF eager path (modeling_llama.py:303-333, ~900 launches per token).
 #include "common.cuh"
@@ -42,7 +42,7 @@ namespace dtk {
 namespace {
 
 constexpr int NCW = 8;                       // consumer warps
-constexpr int NPW = 4;                       // producer warps (one issuing lane each): ~500 cycles per bulk copy
+constexpr int NPW = 4;                       // producer warps (one issuing lane each)
 constexpr int MEGA_THREADS = (NCW + NPW) * 32;
 constexpr int CONSUMER_THREADS = NCW * 32;
 static_assert(NCW % NPW == 0, "slot ownership: NPW must divide NCW");
@@ -99,7 +99,7 @@ DTK_DEV void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMER_T
 // Every activation value that crosses CTAs (residual stream, q, the new key/value row, attention partials and output,
 // the SwiGLU vector) travels as ONE 8-byte word {fp32 value, 32-bit phase tag}: aligned 8-byte accesses are single-copy
 // atomic, so a reader that sees the expected tag also sees the value written with it — no release fence on the
-// producer side (it cost ~0.8 us of every phase) and no acquire on the consumer side. Writers use st.relaxed.gpu.
+// producer side and no acquire on the consumer side. Writers use st.relaxed.gpu.
 // Readers first try a WEAK coalesced load (ld.cg: may be served by the SM's own L2 partition) and only re-read with
 // ld.relaxed.gpu the words whose tag is still old — a stale copy is harmless because it carries a stale tag.
 // The grid-wide counter below is therefore only a HINT that says when reading is worthwhile; correctness rests on the
@@ -136,7 +136,7 @@ struct Spin {   // bounded polling with a short back-off: trap instead of hangin
   uint32_t n = 0;
   long long t0 = 0;
   DTK_DEV void tick() {
-    __nanosleep(32);   // (0 .. 96 ns measured equal, 256 ns +1 %, 512 ns +3 %; pipelined re-polls slower: profiles/r2_decode_poll_sweep.txt)
+    __nanosleep(32);   // short back-off between polls of the same word (not re-tuned on the H100)
     if ((++n & 255u) == 0) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
@@ -216,7 +216,7 @@ DTK_DEV AttnSplit attn_split(const MegaArgs& p, int c, int G, int pos) {
 // where hi = bf16(x), lo = bf16(x - hi). All 8 columns of B are the same vector, so every lane of a quad column reads
 // entry t = lane & 3. Entries for k >= K (padding up to the 256-column tile) are zero.
 //
-// DATAFLOW STAGING (round 2): a tile (group, ks) needs only the 256-element SLICE ks of the vector, so the warp that owns
+// DATAFLOW STAGING: a tile (group, ks) needs only the 256-element SLICE ks of the vector, so the warp that owns
 // the tile stages that slice itself, when it gets there — ONE warp: 4 tagged pairs per lane in one coalesced L2 round trip,
 // re-read coherently until their tags match, converted in registers (the two halves of a B entry meet through one shuffle)
 // and written straight to the entries. No CTA-wide barrier in front of a phase: a warp starts multiplying as soon as ITS
@@ -226,7 +226,7 @@ DTK_DEV AttnSplit attn_split(const MegaArgs& p, int c, int G, int pos) {
 // r = rsqrt(sum over slices / K + eps) is formed by the epilogue warp (same order in every CTA: identical r everywhere).
 // The vector buffer is single: a slice may only be overwritten when every warp of the CTA is past the previous weight
 // phase (phase_done counts warps x phases); the L2 round trip comes first, so that wait is normally free.
-// Inlined (one call site): ptxas ignores setmaxnreg in a kernel that calls functions (C7507); fully inlined measured 0.8 % faster.
+// Inlined (one call site): ptxas ignores setmaxnreg in a kernel that calls functions (C7507).
 DTK_DEV void stage_slice(const u64* src, uint32_t in_tag, bool nowait, const bf16* src_bf16, int K, int ks,
                                          const bf16* norm_w, uint4* xb, float* slice_ss, volatile uint32_t* slice_tag,
                                          uint32_t my_tag) {
@@ -706,7 +706,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
       int since_sync = 0;
       // ---- group epilogues. They do NOT run inside the tile loop: with "the warp that finishes a group's last tile runs its
       // epilogue" the warp that is last in one round starts its next tile late, is last again, and ends up with ALL epilogues of
-      // the phase in series (gate/up: it finished 2 us after the other seven warps, profiles/r2_decode_trace_own_cost.txt). The
+      // the phase in series. The
       // tiles only leave their partial sums in shared memory; after a CTA barrier the complete groups are dealt to the warps
       // (warp w: groups k_ep + w, + 8, ...) and run in parallel — no per-tile counter, atomic or fence either. Partials are
       // summed in k order (deterministic).
@@ -800,7 +800,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
           // part of x, odd columns the lo part (column = lane >> 2), so ONE mma per k-step yields W.hi in accumulator
           // column 0 and W.lo in column 1. The A fragments are loaded in batches interleaved with the mma of earlier
           // batches, so that the tensor pipe starts while the rest of the tile is still being read (shared-memory returns
-          // are in order; all 16 ldmatrix in front of the first mma made the two pipes take turns: 0.53 us per tile).
+          // are in order; all 16 ldmatrix in front of the first mma make the two pipes take turns).
           float rA0, rA2;
           {
             cur_slot = sl;
@@ -863,10 +863,9 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
       stamp(2);
     }
     // Phase boundary: a CTA-wide barrier only (none after qkv: the attention phase meets after polling its head's q; none
-    // after lm_head). No grid-wide arrival counter: the next phase's warps poll the tagged words of their own slices
-    // (0.80 vs 0.91 ms per token with a counter, profiles/r2_decode_variants.txt). The CTA barrier is what allows the single
-    // vector buffer (slices are overwritten by the next phase; the attention merge scratch aliases it), and it is also FASTER
-    // than letting the warps drift (0.788 vs 0.809 ms per token, profiles/r2_decode_ab.txt).
+    // after lm_head). No grid-wide arrival counter: the next phase's warps poll the tagged words of their own slices.
+    // The CTA barrier is what allows the single
+    // vector buffer (slices are overwritten by the next phase; the attention merge scratch aliases it).
     if (ph != PH_QKV && ph != PH_LM) consumer_sync();
     stamp(3);
     if (++ph == 5) { ph = 0; ++l; }

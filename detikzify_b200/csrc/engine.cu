@@ -133,9 +133,9 @@ struct dtk_engine {
   struct VitGraph { cudaGraphExec_t exec; uint64_t launches; };
   std::map<int, VitGraph> vit_graphs;
   float *v_pix_in = nullptr, *v_tok_out = nullptr, *v_pool_out = nullptr;
-  bf16* v_vt = nullptr;      // per-layer V^T copy for the tcgen05 attention
+  bf16* v_vt = nullptr;      // per-layer V^T copy for the wgmma attention
   int vit_graph = 1;
-  int attn_impl = 1;         // ViT attention: 1 = tcgen05 (attn_tc.cu), 0 = mma.sync flash attention (attn_mma.cu)
+  int attn_impl = 1;         // ViT attention: 1 = wgmma (attn_tc.cu), 0 = mma.sync flash attention (attn_mma.cu)
 
   // generation loop
   int gen_B = 0;
@@ -396,7 +396,7 @@ bf16* kv_layer(dtk_engine* eng, int slot, int layer) {
 }
 
 int nsplit_for(const dtk_config& c, int B) {
-  int n = (2 * 148 + c.heads * B - 1) / (c.heads * B);
+  int n = (2 * 132 + c.heads * B - 1) / (c.heads * B);   // two CTAs on each of the H100's 132 SMs
   if (n < 1) n = 1;
   if (n > 16) n = 16;
   return n;
@@ -434,8 +434,8 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
   if (eng->decode_gemm_min_batch > 0 && B >= eng->decode_gemm_min_batch && B <= c.max_len) {
     if (eng->cas_len > 0 && eng->cas_slot >= 0 && nsplit > 4) nsplit = 4;   // cascade: the per-row kernel covers the (short) private suffix only; 12+ partial slots stay for the prefix   // (B rows fit the prefill buffers)
     // ---- batched decode (MCTS rollouts / several figures): the B rows go through the dense matrices as ONE GEMM each, so
-    // the weights are streamed once per step instead of once per sequence (the GEMV kernels below re-read them B times:
-    // measured 59 ms/step for 32 ds-7b rollouts). Activations are rounded to bf16 GEMM operands exactly as in prefill
+    // the weights are streamed once per step instead of once per sequence (the GEMV kernels below re-read them B times).
+    // Activations are rounded to bf16 GEMM operands exactly as in prefill
     // (fp32 residual stream, fp32 accumulation); RoPE / KV append / attention are per row (slot, position).
     const int qkvd = qd + 2 * kd;
     auto gemm = [&](const bf16* A, int K, const bf16* Wm, int N, const float* resid, int glu, float* o32, bf16* o16, int ldo) {
@@ -446,7 +446,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
     };
     // Shared-prefix ("cascade") attention: when every row borrows the same prefix from one slot (MCTS rollouts of a figure),
     // the prefix keys are reduced ONCE per head by the tensor-core flash kernel with the B query rows as its M dimension
-    // (K/V tiles read once instead of B times: 60 -> ~10 us per ds-7b layer at 32 rollouts x 500 shared positions); the
+    // (K/V tiles read once instead of B times); the
     // per-row kernel covers the private suffix only and merges both partial sets.
     const bool cas = eng->cas_len > 0 && eng->cas_slot >= 0;
     const int ctiles_all = cas ? (eng->cas_len + 63) / 64 : 0;
@@ -1209,8 +1209,8 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
     eng->decode_gemm_min_batch = (int)value;
     return DTK_OK;
   }
-  if (std::strcmp(key, "gemm_impl") == 0) {  // process-wide dev switch: 0 = mma.sync, 1 = tcgen05 where supported
-    DTK_REQUIRE(value >= 0 && value <= 3, "gemm_impl must be 0..3");
+  if (std::strcmp(key, "gemm_impl") == 0) {  // process-wide dev switch: 0 = mma.sync, 1 / 2 = wgmma where supported
+    DTK_REQUIRE(value >= 0 && value <= 2, "gemm_impl must be 0..2");
     set_gemm_impl((int)value);
     return DTK_OK;
   }
@@ -1221,10 +1221,6 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
   if (std::strcmp(key, "gemm_swap_split") == 0) {  // process-wide dev switch: split-K factor of the batched-decode GEMM
     DTK_REQUIRE(value >= 0 && value <= 8, "gemm_swap_split must be 0 (heuristic) .. 8");
     set_gemm_swap_split((int)value);
-    return DTK_OK;
-  }
-  if (std::strcmp(key, "gemm_skinny_swap") == 0) {  // process-wide dev switch
-    set_gemm_skinny_swap(value ? 1 : 0);
     return DTK_OK;
   }
   if (std::strcmp(key, "sample_impl") == 0) {  // process-wide: 0 = register-resident sampler when V fits, 1 = generic kernel
@@ -1240,7 +1236,7 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
     eng->mega_debug = value ? 1 : 0;
     return DTK_OK;
   }
-  if (std::strcmp(key, "attn_impl") == 0) {  // ViT attention: 1 (default) = tcgen05, 0 = mma.sync
+  if (std::strcmp(key, "attn_impl") == 0) {  // ViT attention: 1 (default) = wgmma, 0 = mma.sync
     DTK_REQUIRE(value == 0 || value == 1, "attn_impl must be 0 or 1");
     eng->attn_impl = (int)value;
     return DTK_OK;

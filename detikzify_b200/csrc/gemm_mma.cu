@@ -3,7 +3,7 @@
 // Bring-up / small-M tensor path: mma.sync m16n8k16 fed by a 4-stage cp.async ring, 128x128x32
 // tiles, XOR-swizzled shared memory read with ldmatrix. It serves every dense contraction of the
 // path (ViT patch-embed / qkv / out / fc1 / fc2, projector, LLaMA prefill qkv / o / gate-up / down)
-// so the whole engine is correct end to end; the tcgen05/TMA kernel in gemm_tc.cu takes over the
+// so the whole engine is correct end to end; the wgmma/TMA kernel in gemm_tc.cu takes over the
 // large-M shapes (see DESIGN.md "GEMM").
 //
 // Replaces (reference has no native code; these are the library calls it dispatches to):
@@ -156,13 +156,13 @@ __global__ void __launch_bounds__(THREADS) gemm_bf16_tn_kernel(const GemmArgs p)
 
 }  // namespace
 
-static int g_gemm_impl = 2;  // 0 = mma.sync everywhere, 1 = tcgen05 one-tile-per-CTA 128 x 128 kernel, 2 (default) = persistent 128 x 256 tcgen05 kernel, 3 = CTA-pair 256 x 256 kernel (dtk_set_option "gemm_impl")
+static int g_gemm_impl = 2;  // 0 = mma.sync everywhere, 1 = wgmma one-tile-per-CTA 128 x 128 kernel, 2 (default) = persistent 128 x 256 wgmma kernel (dtk_set_option "gemm_impl")
 void set_gemm_impl(int impl) { g_gemm_impl = impl; }
 int get_gemm_impl() { return g_gemm_impl; }
 
 cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
-  // large-M dense contractions go to the tcgen05/TMEM kernel; tiny M (pool head, M = B) stays on mma.sync
-  // (M < 4: pool-head probes and other tiny products stay on mma.sync; 4 <= M < 64 takes the skinny tcgen05 tile)
+  // large-M dense contractions go to the wgmma kernel; tiny M (pool head, M = B) stays on mma.sync
+  // (M < 4: pool-head probes and other tiny products stay on mma.sync; 4 <= M < 64 takes the swapped-operand wgmma tile)
   if (g_gemm_impl >= 1 && a.M >= 4 && gemm_tc_supported(a)) return launch_gemm_tc(a, s, counter);
   return launch_gemm_mma(a, s, counter);
 }

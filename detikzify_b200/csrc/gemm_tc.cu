@@ -1,201 +1,152 @@
-// tcgen05 GEMM  C[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulate in TMEM) — the Blackwell tensor path for
-// the dense contractions of the ViT (qkv / out / fc1+GELU / fc2, patch embed) and the LLaMA prefill (qkv, o, gate/up
-// with SiLU*mul, down), with the same fused epilogues as gemm_mma.cu (bias, GELU, position rows, residual, GLU).
+// wgmma GEMM  C[M,N] = A[M,K] * W[N,K]^T  (bf16 operands, fp32 accumulate in registers) — the Hopper tensor path for the
+// dense contractions of the ViT (qkv / out / fc1+GELU / fc2, patch embed) and the LLaMA prefill (qkv, o, gate/up with
+// SiLU*mul, down), with the same fused epilogues as gemm_mma.cu (bias, GELU, position rows, residual, GLU).
 //
-// One CTA = one 128 x 128 output tile, 192 threads, warp-specialised:
-//   warp 4  TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 128 rows x 64 k) for A and W into a
-//                          3-stage shared-memory ring, mbarrier complete_tx
-//   warp 5  MMA issuer   : one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M128 x N128 x K16) from
-//                          shared-memory descriptors into a 128-column TMEM accumulator; tcgen05.commit releases ring
-//                          slots and finally signals the epilogue
-//   warps 0-3 epilogue   : tcgen05.ld 32x32b (warp w owns TMEM lanes 32w..32w+31 = output rows), epilogue math in
-//                          registers, 128-byte row segments stored to global
-// 96 KB of shared memory and 128 TMEM columns per CTA -> two CTAs per SM, so one tile's epilogue overlaps the other
-// tile's main loop. Out-of-range rows / the K tail are zero-filled by TMA.
-// All mbarrier waits are bounded (trap instead of hanging the GPU).
+// Dense kernel (M >= 64): 128 x BN output tiles, 384 threads, warp-specialised:
+//   warp 8      TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 128 / BN rows x 64 k) for A and W into a
+//                              4-stage shared-memory ring, mbarrier complete_tx; runs ahead across tile boundaries
+//   warps 0-7   two consumer warpgroups: warpgroup g owns rows 64 g .. 64 g + 63 of the tile and issues
+//                              wgmma.mma_async m64nBNk16 from shared-memory descriptors into BN / 2 accumulator registers
+//                              per thread; one k-block stays in flight while the previous ring slot is released;
+//                              epilogue math in registers, stored straight from the accumulator layout
+// setmaxnreg moves registers from the producer warpgroup to the consumers (the 64 x 256 accumulator alone is 128 registers).
+// Out-of-range rows / the K tail are zero-filled by TMA. All mbarrier waits are bounded (trap instead of hanging the GPU).
 #include <cuda.h>
-
-#include <map>
-#include <mutex>
 
 #include "common.cuh"
 #include "launch.h"
+#include "wgmma.cuh"
 
 namespace dtk {
 namespace {
 
 constexpr int TBM = 128, TBK = 64;
-constexpr int TC_THREADS = 192;
 constexpr int A_BYTES = TBM * TBK * 2;                                // 16 KB
-constexpr long long TC_SPIN = 2000000000ll;
-// Two tile shapes: 128 x 128 (3 stages, two CTAs per SM) for M >= 64, and the SKINNY 128 x 32 (8 stages, one CTA per SM)
-// for the batched-decode GEMMs (M = number of rollouts <= 64): there the matrices are streamed once from HBM and what
-// matters is many CTAs (N / 32) with deep TMA pipelines, not tensor throughput.
-template <int TBN, int TSTAGES>
-struct TcCfg {
-  static constexpr int B_BYTES = TBN * TBK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM = TSTAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-};
+constexpr int DSTAGES = 4;
+constexpr int DTHREADS = 384;                                         // two consumer warpgroups + the producer's warpgroup
 
-DTK_DEV void tc_mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count)); }
-DTK_DEV void tc_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory"); }
-DTK_DEV void tc_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  long long t0 = 0;
-  while (!done) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (!done && (++spins & 1023u) == 0) {
-      const long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > TC_SPIN) __trap();
-    }
+template <int BN>
+struct DenseCfg {
+  static constexpr int STAGE_BYTES = A_BYTES + BN * TBK * 2;
+  static constexpr int SMEM = DSTAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+};
+static_assert(DenseCfg<256>::SMEM <= 232448, "dense GEMM shared memory");
+
+DTK_DEV void wgmma_tile(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128k16_ss(d, a, b, acc); }
+DTK_DEV void wgmma_tile(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n256k16_ss(d, a, b, acc); }
+DTK_DEV void wgmma_tile(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n32k16_ss(d, a, b, acc); }
+DTK_DEV void wgmma_tile(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n64k16_ss(d, a, b, acc); }
+
+// 0.5 x (1 + tanh(u)) = x * sigmoid(2u): two MUFU ops instead of the libm tanhf (error ~1e-7 relative, far below bf16 output rounding)
+DTK_DEV float gelu_tanh_fast(float x) {
+  const float u = 0.7978845608028654f * (x + 0.044715f * x * x * x);
+  return __fdividef(x, 1.f + __expf(-2.f * u));
+}
+
+// epilogue of the two adjacent columns (n, n + 1) of row m
+DTK_DEV void dense_store(const GemmArgs& p, int m, int n, float v0, float v1) {
+  if (p.bias) {
+    const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.bias + n));
+    v0 += b.x; v1 += b.y;
   }
-}
-DTK_DEV void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar)
-               : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO=1<<16 |
-// SBO = 1024 B (8 rows x 128 B) >> 4 at bit 32 | version 1 at bit 46 | layout SWIZZLE_128B (2) at bit 61
-DTK_DEV uint64_t umma_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-DTK_DEV void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-DTK_DEV void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
+  if (p.act == ACT_GELU_TANH) { v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1); }
+  else if (p.act == ACT_GELU_ERF) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+  if (p.glu) {
+    const float rr = silu(v0) * v1;
+    const int64_t o = (int64_t)m * p.ldo + (n >> 1);
+    if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
+    else p.out_f32[o] = rr;
+    return;
+  }
+  if (p.rowbias) {
+    const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rowbias + (int64_t)(m % p.rowbias_mod) * p.N + n));
+    v0 += b.x; v1 += b.y;
+  }
+  if (p.resid) {
+    const float2 rs = *reinterpret_cast<const float2*>(p.resid + (int64_t)m * p.ldr + n);
+    v0 += rs.x; v1 += rs.y;
+  }
+  const int64_t o = (int64_t)m * p.ldo + n;
+  if (p.out_bf16) *reinterpret_cast<uint32_t*>(p.out_bf16 + o) = pack_bf16x2(v0, v1);
+  else *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(v0, v1);
 }
 
-struct TcArgs {
-  GemmArgs g;
-};
-
-template <int TBN, int TSTAGES, int MIN_CTAS>
-__global__ void __launch_bounds__(TC_THREADS, MIN_CTAS) gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                       const __grid_constant__ CUtensorMap mapB, const GemmArgs p) {
-  constexpr int STAGE_BYTES = TcCfg<TBN, TSTAGES>::STAGE_BYTES;
+// CTAs walk the output tiles (m fastest: concurrent CTAs share a BN-row band of W) with stride gridDim.x.
+template <int BN>
+__global__ void __launch_bounds__(DTHREADS, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA,
+                                                              const __grid_constant__ CUtensorMap mapB, const GemmArgs p) {
+  constexpr int STAGE_BYTES = DenseCfg<BN>::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sraw = smem_u32(smem_raw);
-  const uint32_t sbase = (sraw + 1023u) & ~1023u;                    // SWIZZLE_128B tiles need 1024-byte alignment
-  const uint32_t bars = sbase + TSTAGES * STAGE_BYTES;              // full[3] empty[3] tmem_full, tmem ptr
-  const uint32_t full0 = bars, empty0 = bars + 8 * TSTAGES, tfull = bars + 16 * TSTAGES, tptr = tfull + 8;
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t full0 = sbase + DSTAGES * STAGE_BYTES, empty0 = full0 + 8 * DSTAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * TBM, n0 = blockIdx.x * TBN;
   const int KT = (p.K + TBK - 1) / TBK;
+  const int MT = (p.M + TBM - 1) / TBM, NT = (p.N + BN - 1) / BN;
+  const int tiles = MT * NT;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TSTAGES; ++s) { tc_mbar_init(full0 + 8 * s, 1); tc_mbar_init(empty0 + 8 * s, 1); }
-    tc_mbar_init(tfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int s = 0; s < DSTAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }   // empty: one arrive per consumer warp
+    mbar_init_fence();
   }
-  if (warp == 5) {  // TMEM allocation: 128 fp32 columns x 128 lanes
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tptr), "n"(TBN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem) : "r"(tptr));
 
-  if (warp == 4) {
-    // ===== TMA producer
-    if (lane == 0) {
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % TSTAGES, use = kt / TSTAGES;
-        if (use > 0) tc_wait(empty0 + 8 * s, (use - 1) & 1);
-        const uint32_t sa = sbase + s * STAGE_BYTES, sb = sa + A_BYTES;
-        tc_expect_tx(full0 + 8 * s, STAGE_BYTES);
-        tma_load_2d(sa, &mapA, kt * TBK, m0, full0 + 8 * s);
-        tma_load_2d(sb, &mapB, kt * TBK, n0, full0 + 8 * s);
-      }
-    }
-  } else if (warp == 5) {
-    // ===== MMA issuer (instruction descriptor: D=F32, A=B=BF16, both K-major, N>>3 at bit 17, M>>4 at bit 24)
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-    if (lane == 0) {
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % TSTAGES, use = kt / TSTAGES;
-        tc_wait(full0 + 8 * s, use & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t sa = sbase + s * STAGE_BYTES, sb = sa + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < TBK / 16; ++k) {
-          // advancing K by 16 elements (32 B) inside the 128-byte swizzle atom = +2 in the (>>4) start-address field
-          umma_f16(tmem, umma_desc(sa + k * 32), umma_desc(sb + k * 32), idesc, (kt | k) != 0);
-        }
-        umma_commit(empty0 + 8 * s);          // frees the ring slot once these MMAs have read it
-      }
-      umma_commit(tfull);                      // accumulator complete
-    }
-  } else {
-    // ===== epilogue warps 0..3: TMEM lanes 32w..32w+31 = rows m0 + 32w + lane
-    tc_wait(tfull, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const int m = m0 + warp * 32 + lane;
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
-    for (int cb = 0; cb < TBN; cb += 32) {
-      uint32_t r[32];
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-            "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-            "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-            "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(trow + (uint32_t)cb));
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      if (m < p.M) {
-        const int nb = n0 + cb;
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const int n = nb + j;
-          if (n >= p.N) break;
-          float v0 = __uint_as_float(r[j]), v1 = __uint_as_float(r[j + 1]);
-          if (p.bias) {
-            const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.bias + n));
-            v0 += b.x; v1 += b.y;
-          }
-          if (p.act == ACT_GELU_TANH) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
-          else if (p.act == ACT_GELU_ERF) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-          if (p.glu) {
-            const float rr = silu(v0) * v1;
-            const int64_t o = (int64_t)m * p.ldo + (n >> 1);
-            if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
-            else p.out_f32[o] = rr;
-            continue;
-          }
-          if (p.rowbias) {
-            const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rowbias + (int64_t)(m % p.rowbias_mod) * p.N + n));
-            v0 += b.x; v1 += b.y;
-          }
-          if (p.resid) {
-            const float2 rs = *reinterpret_cast<const float2*>(p.resid + (int64_t)m * p.ldr + n);
-            v0 += rs.x; v1 += rs.y;
-          }
-          const int64_t o = (int64_t)m * p.ldo + n;
-          if (p.out_bf16) *reinterpret_cast<uint32_t*>(p.out_bf16 + o) = pack_bf16x2(v0, v1);
-          else *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(v0, v1);
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+    if (warp == 8 && lane == 0) {
+      uint32_t it = 0;   // k-blocks issued so far (ring position across tiles)
+      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile % MT) * TBM, n0 = (tile / MT) * BN;
+        for (int kt = 0; kt < KT; ++kt, ++it) {
+          const uint32_t s = it % DSTAGES, use = it / DSTAGES;
+          if (use > 0) mbar_wait(empty0 + 8 * s, (use - 1) & 1);
+          const uint32_t sa = sbase + s * STAGE_BYTES, sb = sa + A_BYTES;
+          mbar_expect_tx(full0 + 8 * s, STAGE_BYTES);
+          tma_load_2d(sa, &mapA, kt * TBK, m0, full0 + 8 * s);
+          tma_load_2d(sb, &mapB, kt * TBK, n0, full0 + 8 * s);
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(TBN));
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+  const int wg = warp >> 2;
+  const int g = lane >> 2, c = lane & 3;
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int m0 = (tile % MT) * TBM, n0 = (tile / MT) * BN;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < KT; ++kt, ++it) {
+      const uint32_t s = it % DSTAGES, use = it / DSTAGES;
+      mbar_wait(full0 + 8 * s, use & 1);
+      const uint32_t sa = sbase + s * STAGE_BYTES + wg * (64 * 128), sb = sbase + s * STAGE_BYTES + A_BYTES;
+      wgmma_acc_fence(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TBK / 16; ++k) wgmma_tile(acc, wgmma_desc(sa + k * 32), wgmma_desc(sb + k * 32), (kt | k) != 0);
+      wgmma_commit();
+      if (kt > 0) {   // the previous k-block has been read: its ring slot goes back to the producer
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(empty0 + 8 * ((it - 1) % DSTAGES));
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_acc_fence(acc);
+    if (lane == 0) mbar_arrive(empty0 + 8 * ((it - 1) % DSTAGES));
+
+    const int r0 = m0 + wg * 64 + (warp & 3) * 16 + g;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * c;
+      if (n >= p.N) break;   // N is even: the pair (n, n + 1) is inside or outside together
+      if (r0 < p.M) dense_store(p, r0, n, acc[4 * j], acc[4 * j + 1]);
+      if (r0 + 8 < p.M) dense_store(p, r0 + 8, n, acc[4 * j + 2], acc[4 * j + 3]);
+    }
   }
 }
 
-// ---- thread-block cluster helpers (split-K reduce of the batched-decode tile, CTA-pair GEMM)
+// ---- thread-block cluster helpers (split-K reduce of the batched-decode tile)
 DTK_DEV uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r)); return r; }
 DTK_DEV void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
@@ -206,372 +157,36 @@ DTK_DEV uint32_t dsmem_addr(uint32_t local_addr, uint32_t rank) {   // same offs
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(ra) : "r"(local_addr), "r"(rank));
   return ra;
 }
-DTK_DEV float4 ld_dsmem_v4(uint32_t cluster_addr) {
-  float4 v;
-  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(cluster_addr));
+DTK_DEV float ld_dsmem(uint32_t cluster_addr) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];\n" : "=f"(v) : "r"(cluster_addr) : "memory");
   return v;
 }
 
-
-// ---- persistent 128 x 256 kernel (gemm_impl = 2): the dense ViT / prefill contractions.
-// One CTA per SM walks the output tiles (m fastest: concurrent CTAs share a 256-row band of W); three pipelines:
-//   warp 8  TMA producer : 4-stage ring of {A 128 x 64, W 256 x 64} SWIZZLE_128B boxes (48 KB per stage), runs ahead across
-//                          tile boundaries
-//   warp 9  MMA issuer   : tcgen05.mma M128 x N256 x K16 into one of TWO 256-column TMEM accumulators (all 512 columns):
-//                          the next tile's main loop starts while the epilogue warps drain the previous accumulator
-//   warps 0-7 epilogue   : tcgen05.ld 32x32b (thread = row) -> padded shared-memory transpose (33-word rows) -> thread =
-//                          COLUMN: bias / activation / position rows / residual / SwiGLU are read and written as whole
-//                          128-byte row segments, eight rows per step as independent dependency chains. (The one-tile
-//                          kernel above stores 8 bytes per thread at row stride — 32 sectors per instruction; a first
-//                          persistent version with four epilogue warps and one row per step was latency-bound in the
-//                          epilogue: ~100 k cycles per tile, 176 TF/s on the ViT qkv shape.)
-// L2 feeds an SM at ~43 B/clk (6300 B/clk chip-wide): a 128 x 256 x 64 step moves 48 KB for 512 tensor-pipe cycles, so this
-// 1-CTA tile tops out near 45 % of the tensor peak; the pair tile (cta_group::2, 256 x 256, W halves shared) is the next step.
-constexpr int PBN = 256, PSTAGES = 4;
-constexpr int PB_BYTES = PBN * TBK * 2;                    // 32 KB
-constexpr int PSTAGE_BYTES = A_BYTES + PB_BYTES;           // 48 KB
-constexpr int PEPI_WARPS = 8;                              // two per TMEM lane quarter: columns [0,128) and [128,256)
-constexpr int PTHREADS = (PEPI_WARPS + 2) * 32;
-constexpr int PSTG_WORDS = 32 * 33;                        // per epilogue warp: 32 rows x 32 columns, padded
-constexpr int PSMEM = PSTAGES * PSTAGE_BYTES + PEPI_WARPS * PSTG_WORDS * 4 + 256 + 1024;
-static_assert(PSMEM <= 232448, "persistent GEMM shared memory");
-
-// 0.5 x (1 + tanh(u)) = x * sigmoid(2u): two MUFU ops instead of the libm tanhf (error ~1e-7 relative, far below bf16 output rounding)
-DTK_DEV float gelu_tanh_fast(float x) {
-  const float u = 0.7978845608028654f * (x + 0.044715f * x * x * x);
-  return __fdividef(x, 1.f + __expf(-2.f * u));
-}
-
-// Epilogue of one 128-row accumulator (shared by the 1-CTA and the CTA-pair persistent kernels): warp w drains TMEM lanes
-// 32 (w % 4) .. + 31 (hardware lane-quarter rule), columns 128 (w / 4) .. + 127 of the 256-column accumulator at `tacc`.
-// `arrive` hands the accumulator back to the MMA issuer (called by lane 0 once this warp's last chunk is in registers).
-template <typename Arrive>
-DTK_DEV void persist_epilogue(const GemmArgs& p, float* stg, uint32_t tacc, int m0, int n0, int warp, int lane, Arrive arrive) {
-  const int quarter = warp & 3, chalf = warp >> 2;
-  const uint32_t trow = tacc + ((uint32_t)(quarter * 32) << 16);
-  const int mrow0 = m0 + quarter * 32;
-  const int nrows = min(32, p.M - mrow0);   // rows of this warp inside the matrix (may be <= 0)
-  const int cb0 = chalf * 128;
-  const int cb1 = min(cb0 + 128, (p.N - n0 + 31) & ~31);   // end of this warp's columns inside the matrix
-  if (cb0 >= cb1) {   // nothing to drain: hand the accumulator back at once
-    __syncwarp();
-    if (lane == 0) arrive();
-    return;
-  }
-#pragma unroll 1
-  for (int cb = cb0; cb < cb1; cb += 32) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(trow + (uint32_t)cb));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-    if (cb + 32 >= cb1) {
-      // this warp's last chunk of the tile is in registers: hand the accumulator back before the stores
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      __syncwarp();
-      if (lane == 0) arrive();
-    }
-#pragma unroll
-    for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(r[j]);   // thread = row: bank (lane + j) % 32
-    __syncwarp();
-    // thread = column n: whole 128-byte row segments from here on; eight rows per step as independent chains
-    const int n = n0 + cb + lane;
-    const bool nin = n < p.N;
-    float bias = 0.f;
-    if (p.bias && nin) bias = __bfloat162float(p.bias[n]);
-#pragma unroll 1
-    for (int rr0 = 0; rr0 < nrows; rr0 += 8) {
-      float v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = stg[(rr0 + u) * 33 + lane] + bias;
-      if (p.act == ACT_GELU_TANH) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v[u] = gelu_tanh_fast(v[u]);
-      } else if (p.act == ACT_GELU_ERF) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v[u] = gelu_erf(v[u]);
-      }
-      if (p.glu) {   // columns (gate, up) are adjacent lanes; out[m, n / 2]
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const float up = __shfl_down_sync(0xffffffffu, v[u], 1);
-          if (!(lane & 1) && nin && rr0 + u < nrows) {
-            const float rv = silu(v[u]) * up;
-            const int64_t o = (int64_t)(mrow0 + rr0 + u) * p.ldo + (n >> 1);
-            if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rv);
-            else p.out_f32[o] = rv;
-          }
-        }
-        continue;
-      }
-      if (p.rowbias) {
-        float t[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u)
-          t[u] = (nin && rr0 + u < nrows) ? __bfloat162float(p.rowbias[(int64_t)((mrow0 + rr0 + u) % p.rowbias_mod) * p.N + n]) : 0.f;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v[u] += t[u];
-      }
-      if (p.resid) {
-        float t[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) t[u] = (nin && rr0 + u < nrows) ? p.resid[(int64_t)(mrow0 + rr0 + u) * p.ldr + n] : 0.f;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v[u] += t[u];
-      }
-      if (p.out_bf16) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const float hi = __shfl_down_sync(0xffffffffu, v[u], 1);
-          if (!(lane & 1) && nin && rr0 + u < nrows)
-            *reinterpret_cast<uint32_t*>(p.out_bf16 + (int64_t)(mrow0 + rr0 + u) * p.ldo + n) = pack_bf16x2(v[u], hi);   // N is even
-        }
-      } else {
-#pragma unroll
-        for (int u = 0; u < 8; ++u)
-          if (nin && rr0 + u < nrows) p.out_f32[(int64_t)(mrow0 + rr0 + u) * p.ldo + n] = v[u];
-      }
-    }
-    __syncwarp();   // the staging tile is rewritten by the next chunk
-  }
-
-}
-
-__global__ void __launch_bounds__(PTHREADS, 1) gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                      const __grid_constant__ CUtensorMap mapB, const GemmArgs p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sraw = smem_u32(smem_raw);
-  const uint32_t sbase = (sraw + 1023u) & ~1023u;
-  const uint32_t stg0 = sbase + PSTAGES * PSTAGE_BYTES;
-  const uint32_t bars = stg0 + PEPI_WARPS * PSTG_WORDS * 4;
-  const uint32_t full0 = bars, empty0 = bars + 8 * PSTAGES, afull0 = bars + 16 * PSTAGES, aempty0 = afull0 + 16, tptr = aempty0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int KT = (p.K + TBK - 1) / TBK;
-  const int MT = (p.M + TBM - 1) / TBM, NT = (p.N + PBN - 1) / PBN;
-  const int tiles = MT * NT;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < PSTAGES; ++s) { tc_mbar_init(full0 + 8 * s, 1); tc_mbar_init(empty0 + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { tc_mbar_init(afull0 + 8 * a, 1); tc_mbar_init(aempty0 + 8 * a, PEPI_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == PEPI_WARPS + 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tptr), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem) : "r"(tptr));
-
-  if (warp == PEPI_WARPS) {
-    if (lane == 0) {
-      uint32_t it = 0;   // k-blocks issued so far (ring position across tiles)
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const int m0 = (tile % MT) * TBM, n0 = (tile / MT) * PBN;
-        for (int kt = 0; kt < KT; ++kt, ++it) {
-          const uint32_t s = it % PSTAGES, use = it / PSTAGES;
-          if (use > 0) tc_wait(empty0 + 8 * s, (use - 1) & 1);
-          const uint32_t sa = sbase + s * PSTAGE_BYTES, sb = sa + A_BYTES;
-          tc_expect_tx(full0 + 8 * s, PSTAGE_BYTES);
-          tma_load_2d(sa, &mapA, kt * TBK, m0, full0 + 8 * s);
-          tma_load_2d(sb, &mapB, kt * TBK, n0, full0 + 8 * s);
-        }
-      }
-    }
-  } else if (warp == PEPI_WARPS + 1) {
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(PBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-    if (lane == 0) {
-      uint32_t it = 0, nt = 0;   // k-blocks / tiles consumed so far
-      for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++nt) {
-        const uint32_t acc = nt & 1, ause = nt >> 1;
-        if (ause > 0) tc_wait(aempty0 + 8 * acc, (ause - 1) & 1);   // the epilogue has drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t tacc = tmem + acc * PBN;
-        for (int kt = 0; kt < KT; ++kt, ++it) {
-          const uint32_t s = it % PSTAGES, use = it / PSTAGES;
-          tc_wait(full0 + 8 * s, use & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-          const uint32_t sa = sbase + s * PSTAGE_BYTES, sb = sa + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TBK / 16; ++k) umma_f16(tacc, umma_desc(sa + k * 32), umma_desc(sb + k * 32), idesc, (kt | k) != 0);
-          umma_commit(empty0 + 8 * s);
-        }
-        umma_commit(afull0 + 8 * acc);
-      }
-    }
-  } else {
-    // ===== epilogue warps 0..7
-    float* stg = reinterpret_cast<float*>(smem_raw + (stg0 - sraw)) + warp * PSTG_WORDS;
-    uint32_t nt = 0;
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++nt) {
-      const uint32_t acc = nt & 1, ause = nt >> 1;
-      const int m0 = (tile % MT) * TBM, n0 = (tile / MT) * PBN;
-      tc_wait(afull0 + 8 * acc, ause & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      const uint32_t bar = aempty0 + 8 * acc;
-      persist_epilogue(p, stg, tmem + acc * PBN, m0, n0, warp, lane,
-                       [bar]() { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory"); });
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (warp == PEPI_WARPS + 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(512));
-  }
-}
-
-// ---- CTA-pair persistent kernel (gemm_impl = 3): tcgen05.mma.cta_group::2, one 256 x 256 output tile per pair of SMs.
-// Each CTA of the pair stages 128 rows of A and HALF of the W tile (128 rows) per k-block — 32 KB instead of the 48 KB the
-// 1-CTA kernel moves for half the flops — and holds its 128 output rows x 256 columns in its own TMEM. Protocol (DeepGEMM /
-// CUTLASS 2-SM layout): both CTAs' TMA loads complete on the LEADER's full barrier (count 2: leader's arrive.expect_tx of
-// both halves' bytes + the peer's remote arrive); the leader's single MMA thread issues for both SMs and commits with
-// multicast to the empty / accumulator-full barriers of BOTH CTAs; the epilogue warps of both CTAs arrive on the leader's
-// accumulator-empty barrier (count 16). Epilogue = persist_epilogue on each CTA's own rows.
-constexpr int QSTAGES = 6;
-constexpr int QSTAGE_BYTES = 2 * A_BYTES;                  // A 128 x 64 + W half 128 x 64 = 32 KB
-constexpr int QSMEM = QSTAGES * QSTAGE_BYTES + PEPI_WARPS * PSTG_WORDS * 4 + 256 + 1024;
-static_assert(QSMEM <= 232448, "pair GEMM shared memory");
-
-DTK_DEV void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t leader_bar) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(leader_bar)
-               : "memory");
-}
-DTK_DEV void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-DTK_DEV void umma_commit_pair(uint32_t bar) {   // arrives on the barrier at this offset in BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(bar), "h"((uint16_t)3)
-               : "memory");
-}
-DTK_DEV void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
-}
-
-__global__ void __launch_bounds__(PTHREADS, 1) gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                                   const __grid_constant__ CUtensorMap mapB, const GemmArgs p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sraw = smem_u32(smem_raw);
-  const uint32_t sbase = (sraw + 1023u) & ~1023u;
-  const uint32_t stg0 = sbase + QSTAGES * QSTAGE_BYTES;
-  const uint32_t bars = stg0 + PEPI_WARPS * PSTG_WORDS * 4;
-  const uint32_t full0 = bars, empty0 = bars + 8 * QSTAGES, afull0 = bars + 16 * QSTAGES, aempty0 = afull0 + 16, tptr = aempty0 + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();   // 0 = leader
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int KT = (p.K + TBK - 1) / TBK;
-  const int MT2 = (p.M + 2 * TBM - 1) / (2 * TBM), NT = (p.N + PBN - 1) / PBN;
-  const int tiles = MT2 * NT;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < QSTAGES; ++s) { tc_mbar_init(full0 + 8 * s, 2); tc_mbar_init(empty0 + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { tc_mbar_init(afull0 + 8 * a, 1); tc_mbar_init(aempty0 + 8 * a, 2 * PEPI_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  cluster_sync_all();   // both CTAs' barriers exist before any remote arrive / multicast commit / 2-SM allocation
-  if (warp == PEPI_WARPS + 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tptr), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  cluster_sync_all();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem) : "r"(tptr));
-
-  if (warp == PEPI_WARPS) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = pair; tile < tiles; tile += npairs) {
-        const int m0 = (tile % MT2) * (2 * TBM) + (int)rank * TBM, n0 = (tile / MT2) * PBN + (int)rank * (PBN / 2);
-        for (int kt = 0; kt < KT; ++kt, ++it) {
-          const uint32_t s = it % QSTAGES, use = it / QSTAGES;
-          if (use > 0) tc_wait(empty0 + 8 * s, (use - 1) & 1);
-          const uint32_t sa = sbase + s * QSTAGE_BYTES, sb = sa + A_BYTES;
-          const uint32_t lbar = dsmem_addr(full0 + 8 * s, 0);   // the leader's full barrier
-          if (rank == 0) tc_expect_tx(full0 + 8 * s, 2 * QSTAGE_BYTES);   // both CTAs' bytes land here
-          else mbar_arrive_cluster(lbar);
-          tma_load_2d_pair(sa, &mapA, kt * TBK, m0, lbar);
-          tma_load_2d_pair(sb, &mapB, kt * TBK, n0, lbar);
-        }
-      }
-    }
-  } else if (warp == PEPI_WARPS + 1) {
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(PBN >> 3) << 17) | ((uint32_t)((2 * TBM) >> 4) << 24);
-    if (lane == 0 && rank == 0) {
-      uint32_t it = 0, nt = 0;
-      for (int tile = pair; tile < tiles; tile += npairs, ++nt) {
-        const uint32_t acc = nt & 1, ause = nt >> 1;
-        if (ause > 0) tc_wait(aempty0 + 8 * acc, (ause - 1) & 1);   // both CTAs' epilogues have drained this accumulator
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t tacc = tmem + acc * PBN;
-        for (int kt = 0; kt < KT; ++kt, ++it) {
-          const uint32_t s = it % QSTAGES, use = it / QSTAGES;
-          tc_wait(full0 + 8 * s, use & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-          const uint32_t sa = sbase + s * QSTAGE_BYTES, sb = sa + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TBK / 16; ++k) umma_f16_pair(tacc, umma_desc(sa + k * 32), umma_desc(sb + k * 32), idesc, (kt | k) != 0);
-          umma_commit_pair(empty0 + 8 * s);
-        }
-        umma_commit_pair(afull0 + 8 * acc);
-      }
-    }
-  } else {
-    float* stg = reinterpret_cast<float*>(smem_raw + (stg0 - sraw)) + warp * PSTG_WORDS;
-    uint32_t nt = 0;
-    for (int tile = pair; tile < tiles; tile += npairs, ++nt) {
-      const uint32_t acc = nt & 1, ause = nt >> 1;
-      const int m0 = (tile % MT2) * (2 * TBM) + (int)rank * TBM, n0 = (tile / MT2) * PBN;
-      tc_wait(afull0 + 8 * acc, ause & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      const uint32_t lbar = dsmem_addr(aempty0 + 8 * acc, 0);
-      persist_epilogue(p, stg, tmem + acc * PBN, m0, n0, warp, lane, [lbar]() { mbar_arrive_cluster(lbar); });
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  cluster_sync_all();   // no CTA of the pair leaves while the other may still signal its barriers
-  if (warp == PEPI_WARPS + 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(512));
-  }
-}
-
-// ---- swapped-operand tile for the batched decode step (M = rollouts <= 64): out[b, n] = sum_k X[b, k] W[n, k].
-// The weight rows are the UMMA M dimension (128 rows of W per CTA, K-major, straight from the arena) and the few batch rows
-// are the N dimension (NB = 32 or 64 columns): per 64-wide k-block a CTA moves 16 KB of weights (bytes that must come from
-// HBM once per step anyway) and only NB x 128 B of activations (L2 resident), instead of a 16 KB activation box that is
-// mostly zero fill next to 4 KB of weights as in the 128 x 32 tile above. The accumulator comes out transposed (TMEM lane =
-// output feature n, column = batch row b): for a fixed b the 32 lanes of a warp store 32 consecutive outputs (coalesced).
-// Epilogue: bias, residual, SwiGLU (gate_i / up_i are adjacent ROWS of W = adjacent lanes: one shuffle), fp32 or bf16 out.
+// ---- swapped-operand tile for the batched decode step (M = rollouts < 64): out[b, n] = sum_k X[b, k] W[n, k].
+// The weight rows are the wgmma M dimension (128 rows of W per CTA, K-major, straight from the arena; warpgroup g takes rows
+// 64 g .. 64 g + 63) and the few batch rows are the N dimension (NB = 32 or 64 columns): per 64-wide k-block a CTA moves
+// 16 KB of weights (bytes that must come from HBM once per step anyway) and only NB x 128 B of activations (L2 resident).
+// The accumulator comes out transposed (row = output feature n, column = batch row b).
+// Epilogue: bias, residual, SwiGLU (gate_i / up_i are adjacent ROWS of W = lanes 4 apart: one shuffle), fp32 or bf16 out.
 //
 // Split-K over a thread-block cluster: a decode GEMM has only N / 128 weight tiles (32 for a 4096-wide projection), far fewer
-// than 2 x 148 CTA slots, and a CTA's bytes in flight are bounded by its ring. `nsplit` CTAs of one cluster share a tile, each
-// streams a contiguous K range into its own TMEM accumulator, ranks > 0 park their fp32 partial tile in their shared memory
+// than 2 x 132 CTA slots, and a CTA's bytes in flight are bounded by its ring. `nsplit` CTAs of one cluster share a tile, each
+// streams a contiguous K range into its own accumulator, ranks > 0 park their fp32 partial tile in their shared memory
 // and rank 0 adds them IN RANK ORDER through distributed shared memory (deterministic) and runs the epilogue. No workspace in
 // HBM, no atomics. Two CTAs per SM (5-stage rings) keep ~200 KB of weights in flight per SM.
+constexpr int STHREADS = 288;   // two consumer warpgroups + the producer warp
 template <int NB, int TSTAGES>
-__global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_swap_kernel(const __grid_constant__ CUtensorMap mapW,
-                                                                    const __grid_constant__ CUtensorMap mapX, const GemmArgs p,
-                                                                    const int nsplit) {
+__global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_constant__ CUtensorMap mapW,
+                                                                  const __grid_constant__ CUtensorMap mapX, const GemmArgs p,
+                                                                  const int nsplit) {
   constexpr int X_BYTES = NB * TBK * 2;
   constexpr int STAGE_BYTES = A_BYTES + X_BYTES;
+  constexpr int NACC = NB / 2;
+  static_assert(NACC * 256 * 4 <= TSTAGES * STAGE_BYTES, "the partial tile is parked in the drained ring");
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sraw = smem_u32(smem_raw);
-  const uint32_t sbase = (sraw + 1023u) & ~1023u;
-  const uint32_t bars = sbase + TSTAGES * STAGE_BYTES;
-  const uint32_t full0 = bars, empty0 = bars + 8 * TSTAGES, tfull = bars + 16 * TSTAGES, tptr = tfull + 8;
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t full0 = sbase + TSTAGES * STAGE_BYTES, empty0 = full0 + 8 * TSTAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = nsplit > 1 ? cluster_ctarank() : 0u;
   const int n0 = (blockIdx.x / nsplit) * TBM;
@@ -579,121 +194,74 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_swap_kernel(const __gri
   const int kt0 = (int)((int64_t)KTall * rank / nsplit), KT = (int)((int64_t)KTall * (rank + 1) / nsplit) - kt0;   // this CTA's k-blocks
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TSTAGES; ++s) { tc_mbar_init(full0 + 8 * s, 1); tc_mbar_init(empty0 + 8 * s, 1); }
-    tc_mbar_init(tfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int s = 0; s < TSTAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }
+    mbar_init_fence();
   }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tptr), "n"(NB));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  uint32_t tmem;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem) : "r"(tptr));
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int kt = 0; kt < KT; ++kt) {
         const int s = kt % TSTAGES, use = kt / TSTAGES;
-        if (use > 0) tc_wait(empty0 + 8 * s, (use - 1) & 1);
+        if (use > 0) mbar_wait(empty0 + 8 * s, (use - 1) & 1);
         const uint32_t sw = sbase + s * STAGE_BYTES, sx = sw + A_BYTES;
-        tc_expect_tx(full0 + 8 * s, STAGE_BYTES);
+        mbar_expect_tx(full0 + 8 * s, STAGE_BYTES);
         tma_load_2d(sw, &mapW, (kt0 + kt) * TBK, n0, full0 + 8 * s);
         tma_load_2d(sx, &mapX, (kt0 + kt) * TBK, 0, full0 + 8 * s);
       }
     }
-  } else if (warp == 5) {
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NB >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-    if (lane == 0) {
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % TSTAGES, use = kt / TSTAGES;
-        tc_wait(full0 + 8 * s, use & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t sw = sbase + s * STAGE_BYTES, sx = sw + A_BYTES;
+  } else {
+    const int wg = warp >> 2;
+    const int g = lane >> 2, c = lane & 3;
+    float acc[NACC];
 #pragma unroll
-        for (int k = 0; k < TBK / 16; ++k) umma_f16(tmem, umma_desc(sw + k * 32), umma_desc(sx + k * 32), idesc, (kt | k) != 0);
-        umma_commit(empty0 + 8 * s);
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < KT; ++kt) {
+      const int s = kt % TSTAGES, use = kt / TSTAGES;
+      mbar_wait(full0 + 8 * s, use & 1);
+      const uint32_t sw = sbase + s * STAGE_BYTES + wg * (64 * 128), sx = sbase + s * STAGE_BYTES + A_BYTES;
+      wgmma_acc_fence(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TBK / 16; ++k) wgmma_tile(acc, wgmma_desc(sw + k * 32), wgmma_desc(sx + k * 32), (kt | k) != 0);
+      wgmma_commit();
+      if (kt > 0) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(empty0 + 8 * ((kt - 1) % TSTAGES));
       }
-      umma_commit(tfull);
     }
-  }
-  // partial tiles of ranks > 0: [128 rows][NB] fp32 in the (drained) ring, a row = one thread's NB values as 16-byte chunks,
-  // chunk index XOR (row & 7): conflict-free 128-bit stores here and 128-bit distributed-shared-memory loads on rank 0
-  const uint32_t prow = sbase + (uint32_t)(warp * 32 + lane) * (NB * 4);
-  const uint32_t psw = (uint32_t)(lane & 7);
-  if (warp < 4 && rank != 0) {
-    tc_wait(tfull, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
-    for (int cb = 0; cb < NB; cb += 32) {
-      uint32_t r[32];
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-            "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-            "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-            "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(trow + (uint32_t)cb));
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+    wgmma_wait<0>();
+    wgmma_acc_fence(acc);
+    // partial tiles of ranks > 0: register i of consumer thread t at word i * 256 + t of the drained ring (both warpgroups
+    // have finished reading it: named barrier over the 256 consumer threads); rank 0's thread t reads the same words
+    const uint32_t pword = sbase + threadIdx.x * 4;
+    if (rank != 0) {
+      asm volatile("bar.sync 1, 256;\n" ::: "memory");
 #pragma unroll
-      for (int c = 0; c < 8; ++c)
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(prow + ((((uint32_t)(cb >> 2) + c) ^ psw) << 4)), "r"(r[4 * c]),
-                     "r"(r[4 * c + 1]), "r"(r[4 * c + 2]), "r"(r[4 * c + 3])
-                     : "memory");
+      for (int i = 0; i < NACC; ++i) asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(pword + i * 1024), "f"(acc[i]) : "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  }
-  if (nsplit > 1) cluster_sync_all();   // partials of every rank are visible to rank 0
-  if (warp < 4 && rank == 0) {
-    // epilogue warps 0..3: TMEM lanes 32w..32w+31 = output features n0 + 32w + lane, columns = batch rows
-    tc_wait(tfull, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const int n = n0 + warp * 32 + lane;
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
-    float bias = 0.f;
-    if (p.bias && n < p.N) bias = __bfloat162float(p.bias[n]);
-#pragma unroll 1
-    for (int cb = 0; cb < NB; cb += 32) {
-      // residual rows of this chunk: all loads in flight before the accumulator is read (one row at a time inside the
-      // store loop below cost 32 dependent L2 round trips, ~10 us of a 30 us o-proj)
-      float rs[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) rs[j] = (p.resid && !p.glu && n < p.N && cb + j < p.M) ? p.resid[(int64_t)(cb + j) * p.ldr + n] : 0.f;
-      uint32_t r[32];
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-            "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-            "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-            "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(trow + (uint32_t)cb));
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      // partial sums of the other ranks, K ranges in order: eight independent 16-byte loads per rank in flight
+    if (nsplit > 1) cluster_sync_all();   // partials of every rank are visible to rank 0
+    if (rank == 0) {
+      // partial sums of the other ranks, K ranges in order
 #pragma unroll 1
       for (uint32_t q = 1; q < (uint32_t)nsplit; ++q) {
-        const uint32_t rrow = dsmem_addr(prow, q);
-        float4 t[8];
+        const uint32_t rword = dsmem_addr(pword, q);
+        float t[NACC];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) t[c] = ld_dsmem_v4(rrow + ((((uint32_t)(cb >> 2) + c) ^ psw) << 4));
+        for (int i = 0; i < NACC; ++i) t[i] = ld_dsmem(rword + i * 1024);
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          r[4 * c] = __float_as_uint(__uint_as_float(r[4 * c]) + t[c].x);
-          r[4 * c + 1] = __float_as_uint(__uint_as_float(r[4 * c + 1]) + t[c].y);
-          r[4 * c + 2] = __float_as_uint(__uint_as_float(r[4 * c + 2]) + t[c].z);
-          r[4 * c + 3] = __float_as_uint(__uint_as_float(r[4 * c + 3]) + t[c].w);
-        }
+        for (int i = 0; i < NACC; ++i) acc[i] += t[i];
       }
+      // rows = output features n (g and g + 8 of this warp's 16), columns = batch rows b
+      const int nA = n0 + wg * 64 + (warp & 3) * 16 + g;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int b = cb + j;            // batch row (warp-uniform)
-        if (b >= p.M) break;
-        float v = __uint_as_float(r[j]) + bias;
+      for (int i = 0; i < NACC; ++i) {
+        const int j = i >> 2, n = nA + ((i & 2) ? 8 : 0), b = 8 * j + 2 * c + (i & 1);
+        float v = acc[i];
+        if (p.bias && n < p.N) v += __bfloat162float(p.bias[n]);
         if (p.glu) {
-          const float other = __shfl_xor_sync(0xffffffffu, v, 1);   // lane pairs (gate, up)
-          if (!(lane & 1) && n + 1 < p.N + 1 && n < p.N) {
+          const float other = __shfl_xor_sync(0xffffffffu, v, 4);   // rows (gate, up) = lanes g, g + 1
+          if (!(g & 1) && n < p.N && b < p.M) {
             const float rr = silu(v) * other;
             const int64_t o = (int64_t)b * p.ldo + (n >> 1);
             if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
@@ -701,22 +269,17 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemm_tc_swap_kernel(const __gri
           }
           continue;
         }
-        if (n < p.N) {
-          v += rs[j];
+        if (n < p.N && b < p.M) {
+          if (p.resid) v += p.resid[(int64_t)b * p.ldr + n];
           const int64_t o = (int64_t)b * p.ldo + n;
           if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(v);
           else p.out_f32[o] = v;
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   }
+  if (warp == 8 && nsplit > 1) cluster_sync_all();   // the producer warp takes part in both cluster barriers
   if (nsplit > 1) cluster_sync_all();   // rank 0 has read every partial: the other CTAs' shared memory may go away
-  __syncthreads();
-  if (warp == 5) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(NB));
-  }
 }
 
 // ---- tensor maps (driver entry point resolved at run time: no link-time dependency on libcuda)
@@ -754,26 +317,34 @@ bool gemm_tc_supported(const GemmArgs& a) {
   if (a.a_rows_per_batch > 0) return false;                       // batched A addressing: mma.sync path
   if ((a.K & 7) || (a.N & 1) || (a.lda & 7) || (a.ldw & 7)) return false;
   if (((uintptr_t)a.A & 15) || ((uintptr_t)a.W & 15)) return false;
+  // the dense epilogue stores column pairs (float2 / packed bf16x2) and reads the residual as float2
+  if (!a.glu && ((a.ldo & 1) || ((uintptr_t)a.out_f32 & 7) || ((uintptr_t)a.out_bf16 & 3))) return false;
+  if (a.resid && ((a.ldr & 1) || ((uintptr_t)a.resid & 7))) return false;
   return encode_fn() != nullptr;
 }
 
-template <int TBN, int TSTAGES, int MIN_CTAS>
-static cudaError_t launch_tc_variant(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
+// persistent = one CTA per SM walks the tiles; otherwise one CTA per tile
+template <int BN>
+static cudaError_t launch_tc_dense(const GemmArgs& a, bool persistent, cudaStream_t s, uint64_t* counter) {
   CUtensorMap mapA, mapB;
-  if (!make_map(&mapA, a.A, a.M, a.K, a.lda, TBM) || !make_map(&mapB, a.W, a.N, a.K, a.ldw, TBN)) return cudaErrorInvalidValue;
-  constexpr int smem = TcCfg<TBN, TSTAGES>::SMEM;
+  if (!make_map(&mapA, a.A, a.M, a.K, a.lda, TBM) || !make_map(&mapB, a.W, a.N, a.K, a.ldw, BN)) return cudaErrorInvalidValue;
+  constexpr int smem = DenseCfg<BN>::SMEM;
   // the attribute is per device; set once per device (not per launch: launches may be captured into a CUDA graph)
   static bool attr_done[64] = {};
+  static int sms[64] = {};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-    e = cudaFuncSetAttribute(gemm_tc_kernel<TBN, TSTAGES, MIN_CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  if (!attr_done[dev]) {
+    e = cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) attr_done[dev] = true;
+    e = cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    attr_done[dev] = true;
   }
-  dim3 grid((a.N + TBN - 1) / TBN, (a.M + TBM - 1) / TBM);
-  gemm_tc_kernel<TBN, TSTAGES, MIN_CTAS><<<grid, TC_THREADS, smem, s>>>(mapA, mapB, a);
+  const int tiles = ((a.M + TBM - 1) / TBM) * ((a.N + BN - 1) / BN);
+  gemm_tc_kernel<BN><<<persistent && tiles > sms[dev] ? sms[dev] : tiles, DTHREADS, smem, s>>>(mapA, mapB, a);
   if (counter) ++*counter;
   return cudaGetLastError();
 }
@@ -795,21 +366,20 @@ static cudaError_t launch_tc_swap(const GemmArgs& a, cudaStream_t s, uint64_t* c
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
-  // split-K factor. A CTA alone pulls ~65 GB/s through its ring (5 stages x 20 KB per ~1.5 us of latency), so about 110
-  // resident CTAs saturate HBM: GEMMs with that many weight tiles are not split (measured: splitting them only adds the
-  // reduction). Projections with few tiles (N = 4096: 32) get the smallest factor that reaches ~110 CTAs, at least 8
+  // split-K factor: GEMMs with about one weight tile per SM or more are not split (splitting them only adds the
+  // reduction). Projections with few tiles (N = 4096: 32) get the smallest factor that reaches ~100 CTAs, at least 8
   // k-blocks per rank.
   const int tiles = (a.N + TBM - 1) / TBM, KT = (a.K + TBK - 1) / TBK;
   int nsplit = 1;
   if (g_swap_split == 0) {
-    while (nsplit < 8 && tiles * nsplit < 110 && KT / (nsplit + 1) >= 8) ++nsplit;
+    while (nsplit < 8 && tiles * nsplit < 100 && KT / (nsplit + 1) >= 8) ++nsplit;
   } else {
     nsplit = g_swap_split;
     while (nsplit > 1 && KT / nsplit < 1) --nsplit;
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(tiles * nsplit));
-  cfg.blockDim = dim3(TC_THREADS);
+  cfg.blockDim = dim3(STHREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
@@ -824,74 +394,15 @@ static cudaError_t launch_tc_swap(const GemmArgs& a, cudaStream_t s, uint64_t* c
   return e;
 }
 
-static cudaError_t launch_tc_persist(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
-  CUtensorMap mapA, mapB;
-  if (!make_map(&mapA, a.A, a.M, a.K, a.lda, TBM) || !make_map(&mapB, a.W, a.N, a.K, a.ldw, PBN)) return cudaErrorInvalidValue;
-  static bool attr_done[64] = {};
-  static int sms[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (!attr_done[dev]) {
-    e = cudaFuncSetAttribute(gemm_tc_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PSMEM);
-    if (e != cudaSuccess) return e;
-    if (cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms[dev] <= 0) sms[dev] = 148;
-    attr_done[dev] = true;
-  }
-  const int tiles = ((a.M + TBM - 1) / TBM) * ((a.N + PBN - 1) / PBN);
-  gemm_tc_persist_kernel<<<tiles < sms[dev] ? tiles : sms[dev], PTHREADS, PSMEM, s>>>(mapA, mapB, a);
-  if (counter) ++*counter;
-  return cudaGetLastError();
-}
-
-static cudaError_t launch_tc_pair(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
-  CUtensorMap mapA, mapB;
-  if (!make_map(&mapA, a.A, a.M, a.K, a.lda, TBM) || !make_map(&mapB, a.W, a.N, a.K, a.ldw, PBN / 2)) return cudaErrorInvalidValue;
-  static bool attr_done[64] = {};
-  static int sms[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-  if (!attr_done[dev]) {
-    e = cudaFuncSetAttribute(gemm_tc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QSMEM);
-    if (e != cudaSuccess) return e;
-    if (cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms[dev] <= 0) sms[dev] = 148;
-    attr_done[dev] = true;
-  }
-  const int tiles = ((a.M + 2 * TBM - 1) / (2 * TBM)) * ((a.N + PBN - 1) / PBN);
-  const int pairs = tiles < sms[dev] / 2 ? tiles : sms[dev] / 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * pairs));
-  cfg.blockDim = dim3(PTHREADS);
-  cfg.dynamicSmemBytes = QSMEM;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, gemm_tc_pair_kernel, mapA, mapB, a);
-  if (counter) ++*counter;
-  return e;
-}
-
-static int g_skinny_swap = 1;   // dev switch (dtk_set_option "gemm_skinny_swap"): 1 = swapped-operand tile for M < 64
-void set_gemm_skinny_swap(int v) { g_skinny_swap = v; }
-
 cudaError_t launch_gemm_tc(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return cudaSuccess;
-  if (a.M < 64 && g_skinny_swap && a.act == ACT_NONE && !a.rowbias) {   // batched decode: weights are the M side
+  if (a.M < 64 && a.act == ACT_NONE && !a.rowbias) {   // batched decode: weights are the M side
     return a.M <= 32 ? launch_tc_swap<32, 5>(a, s, counter) : launch_tc_swap<64, 4>(a, s, counter);
   }
-  if (a.M < 64) return launch_tc_variant<32, 8, 1>(a, s, counter);   // skinny: batched decode
-  if (get_gemm_impl() == 2) return launch_tc_persist(a, s, counter);   // persistent 128 x 256, overlapped epilogue (handing the few-tile
-  // products of the batch-1 ViT to the 128 x 128 kernel was measured: 5.47 vs 4.72 ms per image, rejected)
-  if (get_gemm_impl() == 3) return launch_tc_pair(a, s, counter);      // CTA pairs, 256 x 256, cta_group::2
-  return launch_tc_variant<128, 3, 2>(a, s, counter);
+  // M < 64 with an activation or row bias (pool-head fc1 at M = images per batch) also lands here: the swapped tile has
+  // no such epilogue, so these few small products run on a 128-row tile that is mostly TMA zero fill
+  if (get_gemm_impl() == 2) return launch_tc_dense<256>(a, true, s, counter);   // persistent 128 x 256
+  return launch_tc_dense<128>(a, false, s, counter);
 }
 
 }  // namespace dtk

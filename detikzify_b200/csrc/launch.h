@@ -32,13 +32,12 @@ struct GemmArgs {
   bf16* out_bf16;
   int64_t ldo;
 };
-cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter);   // dispatches tcgen05 / mma.sync
+cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter);   // dispatches wgmma / mma.sync
 cudaError_t launch_gemm_mma(const GemmArgs& a, cudaStream_t s, uint64_t* counter);
 cudaError_t launch_gemm_tc(const GemmArgs& a, cudaStream_t s, uint64_t* counter);
 bool gemm_tc_supported(const GemmArgs& a);
 void set_gemm_swap_split(int v);    // dev: 0 (default) = heuristic split-K factor of the swapped tile, 1..8 = forced
-void set_gemm_skinny_swap(int v);   // dev: 1 (default) = swapped-operand tcgen05 tile for M < 64, 0 = 128 x 32 tile
-void set_gemm_impl(int impl);   // 0 = mma.sync everywhere, 1 = tcgen05 where supported (process-wide dev switch)
+void set_gemm_impl(int impl);   // 0 = mma.sync everywhere, 1 = wgmma one 128 x 128 tile per CTA, 2 = persistent 128 x 256 wgmma (process-wide dev switch)
 int get_gemm_impl();
 
 // ---------------------------------------------------------------- flash attention (mma.sync)
@@ -69,7 +68,7 @@ struct AttnArgs {
 };
 cudaError_t launch_flash_attn(const AttnArgs& a, cudaStream_t s, uint64_t* counter);
 
-// ---------------------------------------------------------------- ViT attention on tcgen05 (attn_tc.cu): head_dim 72, non-causal
+// ---------------------------------------------------------------- ViT attention on wgmma (attn_tc.cu): head_dim 72, non-causal
 // qkv bf16 [B*N, 3*heads*72] (q | k | v column blocks); vT: scratch bf16 [B*heads*80, attn_tc_vt_cols(N)]; o bf16 [B*N, heads*72]
 bool attn_tc_supported();
 int attn_tc_vt_cols(int N);
@@ -222,7 +221,7 @@ struct MegaArgs {
   unsigned long long* amax;                                   // [0] packed (ordered logit, ~index) max cell, [1] arrival counter; zero-initialised, self-resetting
   int *gen_tok, *gen_pos;
   unsigned long long *gen_step, *host_ring;
-  int variant;                                                // dev A/B switches (option "mega_variant"): no switches at present: the round-2 A/B variants were decided, see profiles/r2_decode_ab.txt
+  int variant;                                                // dev A/B switches (option "mega_variant"): no switches at present
   int dbg_flags;                                              // dev only: 1 = skip tile math, 2 = skip grid barriers, 4/8 = relaxed arrive/poll
   long long* dbg;                                             // optional: [grid][5L+1][4] globaltimer stamps (null = off)
   long long* dbg2;                                            // optional: [grid][MEGA_DBG2_ROWS][4] clock64 per-tile trace of layer dbg_layer

@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(256) layernorm_reg_kernel(const float* __restr
 
 // ---- RMSNorm (HF modeling_llama.py:53-67): fp32 x * rsqrt(mean(x^2)+eps) * w
 // One CTA per row: the row stays in registers between the two passes (D <= 4 * 8 * blockDim), every thread has all its
-// loads in flight at once. (One warp per row took 16 us for 32 rows x 4096 on 4 CTAs: 64 dependent load rounds.)
+// loads in flight at once. (One warp per row means 64 dependent load rounds for a 4096-wide row.)
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS) rmsnorm_kernel(const float* __restrict__ x, int64_t ldx,
                                                           const bf16* __restrict__ w, float eps, int M, int D,

@@ -181,7 +181,7 @@ class Engine:
     def __init__(self, cfg: "DetikzifyConfig", arena: torch.Tensor, device: torch.device | int | str = 0,
                  max_seqs: int = 4, max_batch: int = 1, max_len: Optional[int] = None):
         if not torch.cuda.is_available():
-            raise EngineError("detikzify_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise EngineError("detikzify_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load_library()
         self.cfg = cfg
         self.device = torch.device(device if not isinstance(device, int) else f"cuda:{device}")

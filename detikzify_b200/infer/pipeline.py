@@ -13,7 +13,7 @@ Search semantics kept from the reference: one expansion = one rollout from the c
 prefix (same image), a tree node per generated source line, sqrt(n) node thinning, failed-rollout memo
 keyed by token prefix, error-line based pruning, min-max normalised SelfSim reward, widen nodes.
 The rollout runs ``model.generate`` on a worker thread while the caller consumes a TokenStreamer —
-the threading contract of SURVEY.md §8b. What is different underneath: ``model.generate`` is the B200
+the threading contract of SURVEY.md §8b. What is different underneath: ``model.generate`` is the CUDA
 engine (image features cached per figure, KV prefix of the working slot reused, persistent decode
 kernel), so an expansion prefills only the tree-path suffix.
 """

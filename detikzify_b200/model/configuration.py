@@ -1,5 +1,5 @@
 """
-Plain configuration objects for the B200 engine (no HF dependency).
+Plain configuration objects for the CUDA engine (no HF dependency).
 
 Mirrors the attribute names the reference's callers read:
   * ``config.image_token_id`` / ``config.patch_token_id`` and ``config.pooling_mode``

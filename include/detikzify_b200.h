@@ -1,5 +1,5 @@
 /*
- * detikzify_b200 — C ABI of the B200-native engine for DeTikZify's image-conditioned
+ * detikzify_b200 — C ABI of the H100-native (sm_90a) engine for DeTikZify's image-conditioned
  * autoregressive hot path (SigLIP ViT encode -> concat-3 projector -> LLaMA prefill +
  * KV-cached decode + sampler).
  *
@@ -179,7 +179,7 @@ DTK_API int dtk_gen_end(dtk_engine* eng);
 
 /* ---- engine options. "decode_impl": 1 = persistent weight-streaming decode kernel (default for
  *      B = 1), 0 = per-op kernels replayed from a CUDA graph (always used for B > 1). Others (all with
- *      working defaults): "gemm_impl" (see dtk_dbg_gemm_impl), "attn_impl" (ViT attention: 1 = tcgen05, 0 =
+ *      working defaults): "gemm_impl" (see dtk_dbg_gemm_impl), "attn_impl" (ViT attention: 1 = wgmma, 0 =
  *      mma.sync), "cascade_attn" (shared-prefix attention of batched decode), "decode_gemm_min_batch",
  *      "fuse_greedy", "vit_graph", and dev switches "mega_debug", "mega_flags", "mega_trace_layer",
  *      "mega_nslots", "mega_variant". Unknown keys return DTK_ERR_INVALID. ------------------------- */
@@ -203,8 +203,8 @@ DTK_API int dtk_dbg_mega_times(dtk_engine* eng, long long* out_host, int max_val
  * rows 160..164 = the layer's five phases {start, staged, items done, barrier done}; returns the value count */
 DTK_API int dtk_dbg_mega_trace(dtk_engine* eng, long long* out_host, int max_values);
 /* select the dense GEMM implementation used by dtk_dbg_gemm and the engines of this process:
- * 0 = mma.sync, 1 = tcgen05 one 128 x 128 tile per CTA, 2 (default) = persistent 128 x 256 tcgen05 kernel with two TMEM
- * accumulators, 3 = CTA-pair (cta_group::2) 256 x 256 kernel, -1 = query only; returns the current setting. Bits 8..11 of a
+ * 0 = mma.sync, 1 = wgmma one 128 x 128 tile per CTA, 2 (default) = persistent 128 x 256 wgmma kernel,
+ * -1 = query only; returns the current setting. Bits 8..11 of a
  * non-negative value force the split-K factor (cluster size 1..8) of the batched-decode tile; 0 = heuristic. */
 DTK_API int dtk_dbg_gemm_impl(int impl);
 /* C = act(A[M,K] * W[N,K]^T + bias) (+resid); glu: out[m, n/2] = silu(c[m,n]) * c[m,n+1] */
@@ -215,7 +215,7 @@ DTK_API int dtk_dbg_gemm(const void* A_bf16, const void* W_bf16, const void* bia
 DTK_API int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void* o, int B,
                                int heads, int Tq, int Tk, int head_dim, int causal, int q_pos0,
                                float scale, void* stream);
-/* ViT attention on tcgen05: qkv bf16 [B*N, 3*heads*72] (q | k | v column blocks), vt_scratch bf16 [B*heads*80, ceil(N/128)*128],
+/* ViT attention on wgmma: qkv bf16 [B*N, 3*heads*72] (q | k | v column blocks), vt_scratch bf16 [B*heads*80, ceil(N/128)*128],
  * o bf16 [B*N, heads*72]; non-causal, head_dim 72 */
 DTK_API int dtk_dbg_attn_tc(const void* qkv, void* vt_scratch, void* o, int B, int heads, int N, float scale, void* stream);
 /* y = W[N,K] * rmsnorm?(x[K]) ; mode 0 store / 1 add / 2 glu (out[N/2]) */

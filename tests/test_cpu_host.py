@@ -231,12 +231,13 @@ def test_reference_mcts_module_is_drop_in():
     """The reference's vendored MCTS (importable offline) drives our generator unchanged."""
     import importlib.util
     import os
-    base = "/root/reference/detikzify/mcts"
-    if not os.path.isdir(base):
-        pytest.skip("reference checkout not available on this box")
+    base = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "detikzify", "mcts")
+    probe = os.path.join(base, "node.pyc")
+    if not os.path.isfile(probe) or open(probe, "rb").read(4) != importlib.util.MAGIC_NUMBER:
+        pytest.skip("oracle/_ref was not built for this Python (no reference checkout at build time)")
     mods = {}
     for n in ("node", "montecarlo"):
-        spec = importlib.util.spec_from_file_location(f"refmcts_{n}", f"{base}/{n}.py")
+        spec = importlib.util.spec_from_file_location(f"refmcts_{n}", f"{base}/{n}.pyc")
         m = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(m)
         mods[n] = m

@@ -1,15 +1,18 @@
 """
 Drop-in boundary (SURVEY.md §8b): the REFERENCE's own inference driver — detikzify/infer/generate.py (DetikzifyGenerator,
-DetikzifyPipeline, WideNode, rollout streaming), detikzify/mcts/*, detikzify/util/{functools,generation}.py, loaded from
-/root/reference and executed unmodified — runs on top of the objects ``detikzify_b200`` returns (model with ``generate``,
+DetikzifyPipeline, WideNode, rollout streaming), detikzify/mcts/*, detikzify/util/{functools,generation}.py, byte-compiled
+into oracle/_ref by oracle/build_ref.py and executed unmodified — runs on top of the objects ``detikzify_b200`` returns (model with ``generate``,
 processor, tokenizer), with a scripted engine standing in for the GPU. This is the claim "only the ``load`` import changes".
 
 Stubbed because they are absent offline and outside the path: torchmetrics (base class only), the TeX toolchain
 (``infer/tikz.py``: pdf2image / pdfCropMargins / pymupdf → a TikzDocument that "compiles" everything), ``util/image.py``
 (pymupdf, requests → two small PIL helpers), ``model/adapter`` (``has_adapter`` → False), POT's ``emd2`` (v1 models pool
 with "cos"). The reference's ``evaluate/imagesim.py`` (SelfSim reward) is loaded for real on a minimal ``torchmetrics.Metric``.
-Skipped on boxes without the reference checkout (the GPU box).
+Skipped where oracle/_ref was not built (no reference checkout at build time) or was built by another Python version.
+The two tests that compare NUMBERS with the reference (image preprocessing, EMD SelfSim) run everywhere: they compare with
+tests/golden/reference_dropin.npz, which tests/golden/make_reference_dropin_golden.py stored from the reference's own code.
 """
+import contextlib
 import importlib.util
 import os
 import sys
@@ -21,8 +24,20 @@ from PIL import Image, ImageDraw
 
 from scripted_engine import ScriptedEngine
 
-REF = "/root/reference/detikzify"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not available on this box")
+REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "detikzify")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_dropin.npz")
+
+
+def _ref_usable():
+    """oracle/_ref exists and its byte code was compiled by this interpreter version."""
+    probe = os.path.join(REF, "mcts", "node.pyc")
+    if not os.path.isfile(probe):
+        return False
+    with open(probe, "rb") as f:
+        return f.read(4) == importlib.util.MAGIC_NUMBER
+
+
+needs_ref = pytest.mark.skipif(not _ref_usable(), reason="oracle/_ref was not built for this Python (no reference checkout at build time)")
 
 
 def _load(name, path):
@@ -33,8 +48,8 @@ def _load(name, path):
     return mod
 
 
-@pytest.fixture()
-def reference_infer():
+@contextlib.contextmanager
+def reference_modules():
     saved = {k: v for k, v in sys.modules.items() if k.split(".")[0] in ("torchmetrics", "ot", "detikzify")}
     for k in list(saved):
         del sys.modules[k]
@@ -47,10 +62,10 @@ def reference_infer():
             m.__path__ = []
             sys.modules[pkg] = m
         # real reference modules
-        _load("detikzify.mcts.node", f"{REF}/mcts/node.py")
-        _load("detikzify.mcts.montecarlo", f"{REF}/mcts/montecarlo.py")
-        fn = _load("detikzify.util.functools", f"{REF}/util/functools.py")
-        gn = _load("detikzify.util.generation", f"{REF}/util/generation.py")
+        _load("detikzify.mcts.node", f"{REF}/mcts/node.pyc")
+        _load("detikzify.mcts.montecarlo", f"{REF}/mcts/montecarlo.pyc")
+        fn = _load("detikzify.util.functools", f"{REF}/util/functools.pyc")
+        gn = _load("detikzify.util.generation", f"{REF}/util/generation.pyc")
         util = sys.modules["detikzify.util"]
         for mod in (fn, gn):
             for k, v in vars(mod).items():
@@ -69,7 +84,7 @@ def reference_infer():
         sys.modules[adapter.__name__] = adapter
         adapter.AdapterProcessor = type("AdapterProcessor", (), {})
         adapter.CrossAttentionAdapterMixin = type("CrossAttentionAdapterMixin", (), {})
-        _load("detikzify.util.torch", f"{REF}/util/torch.py")
+        _load("detikzify.util.torch", f"{REF}/util/torch.pyc")
         util.infer_device = sys.modules["detikzify.util.torch"].infer_device
         # torchmetrics.Metric: the slice of its protocol the reference's ImageSim relies on (states, reset, device/dtype)
         class Metric(torch.nn.Module):
@@ -113,7 +128,7 @@ def reference_infer():
             return float(res.fun)
         otlp.emd2 = emd2
         sys.modules["ot"], sys.modules["ot.lp"] = ot, otlp
-        _load("detikzify.evaluate.imagesim", f"{REF}/evaluate/imagesim.py")
+        _load("detikzify.evaluate.imagesim", f"{REF}/evaluate/imagesim.pyc")
         tikz = types.ModuleType("detikzify.infer.tikz")
 
         class TikzDocument:
@@ -128,11 +143,17 @@ def reference_infer():
                 return Image.new("RGB", (32, 32), "white")
         tikz.TikzDocument = TikzDocument
         sys.modules[tikz.__name__] = tikz
-        yield _load("detikzify.infer.generate", f"{REF}/infer/generate.py")
+        yield _load("detikzify.infer.generate", f"{REF}/infer/generate.pyc")
     finally:
         for k in [k for k in sys.modules if k.split(".")[0] in ("torchmetrics", "ot", "detikzify")]:
             del sys.modules[k]
         sys.modules.update(saved)
+
+
+@pytest.fixture()
+def reference_infer():
+    with reference_modules() as mod:
+        yield mod
 
 
 def _ours(eos_at=40):
@@ -151,6 +172,7 @@ def _figure(size=90):
     return im
 
 
+@needs_ref
 def test_reference_pipeline_sample_runs_on_our_model(reference_infer):
     model, proc, eng = _ours(eos_at=30)
     pipe = reference_infer.DetikzifyPipeline(model=model, processor=proc, metric="fast")
@@ -163,6 +185,7 @@ def test_reference_pipeline_sample_runs_on_our_model(reference_infer):
     assert kw["do_sample"] and abs(kw["temperature"] - 0.8) < 1e-6 and abs(kw["top_p"] - 0.95) < 1e-6
 
 
+@needs_ref
 def test_reference_mcts_simulate_runs_on_our_model(reference_infer):
     model, proc, eng = _ours(eos_at=36)
     pipe = reference_infer.DetikzifyPipeline(model=model, processor=proc, metric="fast")
@@ -174,6 +197,7 @@ def test_reference_mcts_simulate_runs_on_our_model(reference_infer):
     assert sum(1 for c in eng.calls if c[0] == "gen_begin") >= 4
 
 
+@needs_ref
 def test_reference_generator_abort_and_tree(reference_infer):
     model, proc, eng = _ours(eos_at=60)
     gen = reference_infer.DetikzifyGenerator(model=model, processor=proc, image=_figure(), metric=None,
@@ -187,6 +211,7 @@ def test_reference_generator_abort_and_tree(reference_infer):
     assert gen.newlineinfo and all(v.num_lines >= 1 for v in gen.newlineinfo.values())
 
 
+@needs_ref
 def test_reference_selfsim_metric_runs_on_our_vision_model(reference_infer):
     """metric="model": the reference's ImageSim.from_detikzify wraps OUR model.model.vision_model / image processor and
     computes the SelfSim reward from pooler_output (evaluate/imagesim.py:60-125); MCTS then min-max-normalises it."""
@@ -201,33 +226,38 @@ def test_reference_selfsim_metric_runs_on_our_vision_model(reference_infer):
     assert any(c[0] == "vit_encode" for c in eng.calls)
 
 
-def test_reference_emd_selfsim_agrees_with_ours(reference_infer):
-    """The v2 default reward: the reference's own ImageSim in "emd" mode (evaluate/imagesim.py:105-107,121-123; POT's emd2
-    restated as the transport LP) and ours (assignment solver) on the same vision model object and image processor."""
-    from PIL import ImageDraw
-    from detikzify_b200.evaluate.imagesim import ImageSim as Ours
-    RefImageSim = sys.modules["detikzify.evaluate.imagesim"].ImageSim
-    model, proc, eng = _ours(eos_at=36)
-    ref = RefImageSim.from_detikzify(model, proc, mode="emd")
-    ours = Ours.from_detikzify(model, proc, mode="emd")
+def _other_figure():
     other = Image.new("RGB", (80, 80), "white")
     ImageDraw.Draw(other).ellipse((10, 10, 60, 70), outline="black", width=4)
-    # the reference object feeds bf16 pixels (its .to(device, dtype)), ours fp32: compare the solvers on the SAME patch tokens ...
-    f1, f2 = ref.get_vision_features(_figure()), ref.get_vision_features(other)
-    a = ref.get_similarity(_figure(), other)
-    assert f1.ndim == 2 and a == pytest.approx(Ours._emd_similarity(f1, f2), abs=1e-9) and -1.0 < a < 1.0
-    # ... and the two end-to-end paths within the bf16 rounding of the inputs
-    assert a == pytest.approx(ours.get_similarity(_figure(), other), abs=5e-2)
-    assert ref.get_similarity(_figure(), _figure()) == pytest.approx(1.0, abs=1e-9)
+    return other
 
 
-def test_image_processor_matches_reference_preprocess():
-    """§8 row a1: our host-side DetikzifyImageProcessor against the reference's own class
-    (detikzify/model/v1/processing_detikzify.py:162-253, loaded from /root/reference; only ``timm.data`` / ``timm.models``,
-    which its ``from_pretrained`` would consult for the SigLIP data config, are stubbed). The instance is built from the
-    dict ``from_pretrained`` assembles (:104-117) with timm's published config of vit_so400m_patch14_siglip_384:
-    input 3x384x384, mean = std = 0.5, bicubic."""
+def _preprocess_images():
     import numpy as np
+    rng = np.random.default_rng(3)
+    return [_figure(90), _figure(384).resize((384, 384)), Image.fromarray(rng.integers(0, 255, (200, 311, 3), dtype=np.uint8))]
+
+
+def _pixel_sample(n):
+    """Fixed, seeded sample of the 3 x 384 x 384 pixel values (the golden file stores these positions only)."""
+    import numpy as np
+    return np.random.default_rng(11).choice(3 * 384 * 384, size=n, replace=False)
+
+
+def reference_emd_case():
+    """Runs the REFERENCE's ImageSim in "emd" mode on our vision model -> (patch tokens of both figures, its similarities)."""
+    with reference_modules():
+        RefImageSim = sys.modules["detikzify.evaluate.imagesim"].ImageSim
+        model, proc, _ = _ours(eos_at=36)
+        ref = RefImageSim.from_detikzify(model, proc, mode="emd")
+        f1, f2 = ref.get_vision_features(_figure()), ref.get_vision_features(_other_figure())
+        return f1, f2, ref.get_similarity(_figure(), _other_figure()), ref.get_similarity(_figure(), _figure())
+
+
+def reference_preprocess_case():
+    """Runs the REFERENCE's DetikzifyImageProcessor (only ``timm.data`` / ``timm.models``, which its ``from_pretrained`` would
+    consult for the SigLIP data config, are stubbed with timm's published config of vit_so400m_patch14_siglip_384:
+    input 3x384x384, mean = std = 0.5, bicubic) -> (its attributes, pixel_values per test image)."""
     saved = {k: v for k, v in sys.modules.items() if k.split(".")[0] == "timm"}
     try:
         timm = types.ModuleType("timm"); timm.__path__ = []
@@ -236,21 +266,56 @@ def test_image_processor_matches_reference_preprocess():
         models.resolve_pretrained_cfg = lambda variant: types.SimpleNamespace(to_dict=lambda: dict(cfg))
         data.resolve_data_config = lambda d: dict(d)
         sys.modules.update({"timm": timm, "timm.data": data, "timm.models": models})
-        ref_mod = _load("ref_processing_detikzify", f"{REF}/model/v1/processing_detikzify.py")
+        ref_mod = _load("ref_processing_detikzify", f"{REF}/model/v1/processing_detikzify.pyc")
         ref = ref_mod.DetikzifyImageProcessor.from_pretrained("vit_so400m_patch14_siglip_384.webli")
     finally:
         for k in [k for k in sys.modules if k.split(".")[0] == "timm"]:
             del sys.modules[k]
         sys.modules.update(saved)
         sys.modules.pop("ref_processing_detikzify", None)
+    attrs = [float(ref.size["height"]), float(ref.size["width"]), *map(float, ref.image_mean), *map(float, ref.image_std),
+             float(int(ref.resample)), float(ref.rescale_factor)]
+    return attrs, [ref(images=im, return_tensors="pt")["pixel_values"].float() for im in _preprocess_images()]
+
+
+def test_reference_emd_selfsim_agrees_with_ours():
+    """The v2 default reward: the reference's own ImageSim in "emd" mode (evaluate/imagesim.py:105-107,121-123; POT's emd2
+    restated as the transport LP) and ours (assignment solver) on the same vision model object and image processor. The
+    reference side is stored (patch tokens it extracted and the similarities it computed) and re-run live where oracle/_ref
+    is available."""
+    import numpy as np
+    from detikzify_b200.evaluate.imagesim import ImageSim as Ours
+    g = np.load(GOLDEN)
+    cases = [(torch.from_numpy(g["emd_f1"]), torch.from_numpy(g["emd_f2"]), float(g["emd_sim"]), float(g["emd_self"]))]
+    if _ref_usable():
+        cases.append(reference_emd_case())
+    model, proc, eng = _ours(eos_at=36)
+    ours = Ours.from_detikzify(model, proc, mode="emd")
+    for f1, f2, a, a_self in cases:
+        # the reference object feeds bf16 pixels (its .to(device, dtype)), ours fp32: compare the solvers on the SAME patch tokens ...
+        assert f1.ndim == 2 and a == pytest.approx(Ours._emd_similarity(f1.float(), f2.float()), abs=1e-9) and -1.0 < a < 1.0
+        # ... and the two end-to-end paths within the bf16 rounding of the inputs
+        assert a == pytest.approx(ours.get_similarity(_figure(), _other_figure()), abs=5e-2)
+        assert a_self == pytest.approx(1.0, abs=1e-9)
+
+
+def test_image_processor_matches_reference_preprocess():
+    """§8 row a1: our host-side DetikzifyImageProcessor against the reference's own class
+    (detikzify/model/v1/processing_detikzify.py:162-253): its attributes and a fixed sample of 60 000 of the pixel values it
+    produced per test image are stored; where oracle/_ref is available the class is also run live on every pixel."""
+    import numpy as np
     from detikzify_b200.model.processing import DetikzifyImageProcessor
     ours = DetikzifyImageProcessor(size=384)
-    assert ref.size == ours.size and list(ref.image_mean) == ours.image_mean and list(ref.image_std) == ours.image_std
-    assert int(ref.resample) == ours.resample == 3 and abs(ref.rescale_factor - ours.rescale_factor) < 1e-12
-    rng = np.random.default_rng(3)
-    images = [_figure(90), _figure(384).resize((384, 384)), Image.fromarray(rng.integers(0, 255, (200, 311, 3), dtype=np.uint8))]
-    for im in images:
-        a = ref(images=im, return_tensors="pt")["pixel_values"]
-        b = ours(im, return_tensors="pt")["pixel_values"]
-        assert a.shape == b.shape == (1, 3, 384, 384) and b.dtype == torch.float32
-        assert (a.float() - b).abs().max().item() < 1e-6
+    mine = [float(ours.size["height"]), float(ours.size["width"]), *ours.image_mean, *ours.image_std, float(ours.resample), ours.rescale_factor]
+    g = np.load(GOLDEN)
+    assert np.allclose(g["proc_attrs"], mine, rtol=0, atol=1e-12) and ours.resample == 3
+    idx = _pixel_sample(g["proc_pixels"].shape[1])
+    outs = [ours(im, return_tensors="pt")["pixel_values"] for im in _preprocess_images()]
+    for b, want in zip(outs, g["proc_pixels"]):
+        assert b.shape == (1, 3, 384, 384) and b.dtype == torch.float32
+        assert np.abs(b.reshape(-1).numpy()[idx] - want).max() < 1e-6
+    if _ref_usable():
+        attrs, ref_outs = reference_preprocess_case()
+        assert np.allclose(attrs, mine, rtol=0, atol=1e-12)
+        for a, b in zip(ref_outs, outs):
+            assert a.shape == b.shape and (a - b).abs().max().item() < 1e-6

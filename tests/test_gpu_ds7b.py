@@ -3,7 +3,7 @@ BASELINE.json configs[3]/[4] shapes: every detikzify-ds-7b matrix shape (H 4096,
 decoder layers ("ds-7b-2l", so the fp32 CPU oracle fits and finishes in seconds) —
   * prefill last-row logits,
   * batch-1 decode on the persistent kernel and on the per-op kernels (teacher-forced),
-  * the batched-GEMM decode step every B >= 4 rollout step takes (skinny tcgen05 tile at K = 4096 / 11008), B = 32 ragged
+  * the batched-GEMM decode step every B >= 4 rollout step takes (swapped-operand wgmma tile at K = 4096 / 11008), B = 32 ragged
     contexts, two consecutive steps (the second reads the KV rows the first appended),
   * the nucleus sampler's post-processor probability vector on those batched logits (T 0.8, top-p 0.95: configs[3]),
 all against oracle/hf_oracle.py.
@@ -11,8 +11,8 @@ all against oracle/hf_oracle.py.
 Tolerance: logits max-abs <= 8 % of the reference logits' RMS (and never below the 3e-2 used at |logits| ~ 1). With two
 layers the random-init fixture is dominated by the image rows (projector outputs of O(1) per element next to 0.02-scale
 token embeddings), and the bf16 KV cache / bf16 GEMM operands put 4-5 % of the logits' RMS of noise on BOTH decode
-implementations alike (profiles/r2_parity_diag_7b.txt: persistent vs per-op kernels differ by 6e-4, each is 0.05-0.07 from
-the fp32 oracle at |logits| rms 1.28, max 6.9); greedy ids must still agree wherever the oracle's margin exceeds 2x that.
+implementations alike (tools/diag_parity.py prints the split: persistent vs per-op kernels agree far more closely with each
+other than either does with the fp32 oracle); greedy ids must still agree wherever the oracle's margin exceeds 2x that.
 """
 import pytest
 import torch

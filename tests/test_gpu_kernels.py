@@ -42,10 +42,10 @@ GEMM_SHAPES = [
     (1, 1152, 1152, True, 0, False, False, False),      # M = 1 (pool head probe)
     (130, 264, 72, False, 0, False, False, False),      # ragged everything
     (300, 32256, 256, False, 0, False, False, False),   # wide N (lm_head all-logits path)
-    (5832, 4304, 1152, True, 1, False, False, True),    # ViT fc1 at B = 8: 782 tiles of 128 x 256 over 148 persistent CTAs
+    (5832, 4304, 1152, True, 1, False, False, True),    # ViT fc1 at B = 8: 782 tiles of 128 x 256 over 132 persistent CTAs
     (5832, 1152, 4304, True, 0, True, False, False),    # ViT fc2 at B = 8 (fp32 out + residual, ragged K)
     (2047, 11008, 2048, False, 0, False, True, True),   # prefill gate/up at the 2k context (GLU, bf16 out)
-    # batched decode (M = number of rollouts): the skinny 128 x 32 tcgen05 tile
+    # batched decode (M = number of rollouts): the swapped-operand wgmma tile
     (32, 6144, 2048, False, 0, False, False, False),    # qkv, 32 rollouts
     (32, 2048, 5504, False, 0, True, False, False),     # down + residual, ragged K tile
     (17, 11008, 2048, False, 0, False, True, True),     # gate/up GLU, odd M
@@ -58,8 +58,8 @@ GEMM_SHAPES = [
 @pytest.mark.parametrize("impl", [0, 1, 2], ids=["mma_sync", "tcgen05", "tcgen05_persistent"])
 @pytest.mark.parametrize("M,N,K,bias,act,resid,glu,obf", GEMM_SHAPES)
 def test_gemm_matches_torch(M, N, K, bias, act, resid, glu, obf, impl):
-    """The dense-GEMM implementations (mma.sync bring-up kernel, one-tile tcgen05/TMA/TMEM kernel, persistent 128 x 256
-    tcgen05 kernel with two TMEM accumulators and the transposing epilogue) against torch fp32."""
+    """The dense-GEMM implementations (mma.sync bring-up kernel, one-tile 128 x 128 wgmma/TMA kernel, persistent 128 x 256
+    wgmma kernel; the parameter ids keep their historical names) against torch fp32."""
     prev = _lib().dtk_dbg_gemm_impl(-1)
     _lib().dtk_dbg_gemm_impl(impl)
     try:
@@ -69,7 +69,7 @@ def test_gemm_matches_torch(M, N, K, bias, act, resid, glu, obf, impl):
 
 
 SPLIT_SHAPES = [
-    # (M, N, K, bias, resid, glu, out_bf16): the batched-decode tile (weights as the UMMA M side) with cluster split-K
+    # (M, N, K, bias, resid, glu, out_bf16): the batched-decode tile (weights as the wgmma M side) with cluster split-K
     (32, 4096, 4096, False, True, False, False),      # 7b o-proj + residual
     (32, 4096, 11008, False, True, False, False),     # 7b down + residual
     (32, 22016, 4096, False, False, True, True),      # 7b gate/up GLU
@@ -158,7 +158,7 @@ def test_flash_attention_matches_torch(B, heads, Tq, Tk, D, causal, q_pos0):
 
 @pytest.mark.parametrize("B,heads,N", [(2, 16, 729), (1, 2, 16), (3, 3, 81), (1, 16, 900), (5, 4, 130), (64, 16, 729)])
 def test_tcgen05_vit_attention_matches_torch(B, heads, N):
-    """attn_tc.cu: the ViT attention on tcgen05 (fused qkv layout in, head_dim 72 padded to 80 by TMA zero fill, ragged last
+    """attn_tc.cu: the ViT attention on wgmma (fused qkv layout in, head_dim 72 padded to 80 by TMA zero fill, ragged last
     key block masked) against fp32 softmax attention of the same bf16 inputs; 729 = v1 tower, 900 = v2 tower."""
     torch.manual_seed(B * 31 + N)
     dev, D = "cuda", heads * 72
@@ -214,17 +214,3 @@ def test_decode_gemv_matches_torch(N, K, mode, norm):
     assert rc == 0
     torch.cuda.synchronize()
     torch.testing.assert_close(out, ref, rtol=2e-3, atol=2e-3)
-
-
-# Last in the file on purpose: a protocol error in the CTA-pair kernel traps (bounded waits) and poisons the CUDA context of
-# this process; nothing else may depend on it.
-@pytest.mark.parametrize("M,N,K,bias,act,resid,glu,obf", [c for c in GEMM_SHAPES if c[0] >= 64])
-def test_gemm_cta_pair_matches_torch(M, N, K, bias, act, resid, glu, obf):
-    """tcgen05.mma.cta_group::2: 256 x 256 tiles on pairs of SMs, W halves staged by each CTA of the pair, multicast commits
-    (gemm_impl 3), against torch fp32 on every dense shape of the path."""
-    prev = _lib().dtk_dbg_gemm_impl(-1)
-    _lib().dtk_dbg_gemm_impl(3)
-    try:
-        _gemm_case(M, N, K, bias, act, resid, glu, obf)
-    finally:
-        _lib().dtk_dbg_gemm_impl(prev)

@@ -1,5 +1,5 @@
 """
-Oracle-backed parity of the paths round 1 only checked against the engine itself (VERDICT r1, "parity holes"):
+Oracle-backed parity of paths that would otherwise only be checked against the engine itself:
   * image span in the MIDDLE of the prompt through dtk_prefill, against the logits the REFERENCE's own
     DetikzifyForCausalLM produced (tests/golden/reference_v1_tiny.pt, detikzify/model/v1/modeling_detikzify.py:157-200);
   * dtk_seq_fork and suffix prefill against oracle.forward_logits;

@@ -1,4 +1,4 @@
-"""BASELINE.json configs[3] shape check (dev tool, GPU box): detikzify-ds-7b random-init, (1) batch-1 decode: persistent kernel
+"""BASELINE.json configs[3] shape check (dev tool): detikzify-ds-7b random-init, (1) batch-1 decode: persistent kernel
 vs per-op kernels (logits agreement, ms/token), (2) 32 parallel rollouts with nucleus sampling through the fused generation
 loop (CUDA graph of per-op kernels): tokens/s, and batched-vs-single logits agreement."""
 import sys, time

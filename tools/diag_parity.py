@@ -1,4 +1,4 @@
-"""Where does the logits error of a model shape come from? (dev tool; GPU box) prefill last row, batch-1 decode on the
+"""Where does the logits error of a model shape come from? (dev tool) prefill last row, batch-1 decode on the
 persistent kernel and on the per-op kernels, each against the fp32 oracle; plus persistent vs per-op."""
 import sys
 import torch

@@ -1,5 +1,5 @@
-"""Dense-GEMM timing at the model shapes (mma.sync kernel vs tcgen05 kernel) + ViT / prefill wall time per implementation.
-Dev tool, run on the GPU box:  python tools/gemm_bench.py [model]"""
+"""Dense-GEMM timing at the model shapes (mma.sync kernel vs the wgmma kernels) + ViT / prefill wall time per implementation.
+Dev tool:  python tools/gemm_bench.py [model]"""
 import ctypes as C, math, sys
 import torch
 sys.path.insert(0, ".")
@@ -15,7 +15,7 @@ SHAPES = [  # (M, N, K, out_bf16, label)
     (243, 6144, 2048, False, "llama qkv T=243"), (243, 11008, 2048, True, "llama gate/up T=243"), (243, 2048, 5504, False, "llama down T=243"),
     (2048, 6144, 2048, False, "llama qkv T=2048"), (2048, 11008, 2048, True, "llama gate/up T=2048"), (2048, 2048, 5504, False, "llama down T=2048"),
 ]
-IMPLS = [int(v) for v in sys.argv[2].split(",")] if len(sys.argv) > 2 else [0, 1, 2]   # 3 = CTA pair
+IMPLS = [int(v) for v in sys.argv[2].split(",")] if len(sys.argv) > 2 else [0, 1, 2]
 ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 for M, N, K, obf, label in SHAPES:
     A = (torch.randn(M, K, device="cuda") * 0.5).bfloat16()
@@ -33,7 +33,7 @@ for M, N, K, obf, label in SHAPES:
         ev1.record(); torch.cuda.synchronize()
         us = ev0.elapsed_time(ev1) / 20 * 1e3
         res.append((us, 2.0 * M * N * K / us / 1e6))
-    print(f"{label:24s} M={M:5d} N={N:5d} K={K:5d}  mma.sync {res[0][0]:8.1f} us {res[0][1]:7.1f} TF/s | tcgen05 {res[1][0]:8.1f} us {res[1][1]:7.1f} TF/s | persistent {res[2][0]:8.1f} us {res[2][1]:7.1f} TF/s" + (f" | cta pair {res[3][0]:8.1f} us {res[3][1]:7.1f} TF/s" if len(res) > 3 else ""))
+    print(f"{label:24s} M={M:5d} N={N:5d} K={K:5d}  mma.sync {res[0][0]:8.1f} us {res[0][1]:7.1f} TF/s | wgmma 128x128 {res[1][0]:8.1f} us {res[1][1]:7.1f} TF/s | persistent {res[2][0]:8.1f} us {res[2][1]:7.1f} TF/s")
 
 name = sys.argv[1] if len(sys.argv) > 1 else "nllg/detikzify-ds-1.3b"
 model, _ = load(name, device_map=0)

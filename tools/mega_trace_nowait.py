@@ -21,7 +21,8 @@ eng.set_option("mega_trace_layer", TL)
 for _ in range(3):
     eng.decode([slot], [ctx], tok)
 torch.cuda.synchronize()
-ROWS, G, MHZ = 168, 148, 1965.0
+props = torch.cuda.get_device_properties(0)
+ROWS, G, MHZ = 168, props.multi_processor_count, props.clock_rate / 1e3   # one CTA per SM; SM clock at its maximum
 buf2 = (C.c_longlong * (G * ROWS * 4))()
 got = eng.lib.dtk_dbg_mega_trace(eng._h, buf2, G * ROWS * 4)
 tr = torch.tensor(list(buf2[:got]), dtype=torch.float64).view(-1, ROWS, 4)

@@ -1,4 +1,4 @@
-"""Streaming-primitive microbenchmark (dev tool; run on the GPU box).
+"""Streaming-primitive microbenchmark (dev tool).
 
 Builds tools/csrc/stream_bench.cu into tools/libdtk_dev.so (NOT part of the product library) and measures
 how fast persistent CTAs pull a large buffer from HBM: chip-wide, and per SM when only `grid` CTAs run
@@ -15,7 +15,7 @@ def build():
     src = ROOT / "csrc" / "stream_bench.cu"
     if LIB.exists() and LIB.stat().st_mtime > src.stat().st_mtime:
         return LIB
-    cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
            "-shared", "-Xcompiler", "-fPIC", "-o", str(LIB), str(src)]
     subprocess.run(cmd, check=True)
     return LIB
@@ -34,7 +34,7 @@ if __name__ == "__main__":
     sink = torch.zeros(4, device="cuda")
     s = C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
-    def run(mode, chunk, nslots, ncw, npw, read, hint, grid=148, iters=5, nb=nbytes):
+    def run(mode, chunk, nslots, ncw, npw, read, hint, grid=132, iters=5, nb=nbytes):
         args = (C.c_void_p(buf.data_ptr()), nb, mode, chunk, nslots, ncw, npw, read, hint, grid, C.c_void_p(sink.data_ptr()), s)
         rc = lib.dtk_dbg_stream_bench(*args)
         assert rc == 0, rc
@@ -48,7 +48,7 @@ if __name__ == "__main__":
 
     quick = len(sys.argv) > 1 and sys.argv[1] == "quick"
     print("per-SM ingest when only `grid` CTAs stream (GB/s total | GB/s per SM):")
-    for grid in (1, 2, 8, 32, 74, 111, 148):
+    for grid in (1, 2, 8, 32, 66, 99, 132):
         nb = min(nbytes, grid * 96 * 2**20)
         row = [f"grid {grid:3d}:"]
         for label, a in (("tma 8K x24 p4", (0, 8192, 24, 8, 4, 1, 0)), ("tma 8K x24 p8", (0, 8192, 24, 8, 8, 1, 0)),

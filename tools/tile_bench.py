@@ -1,4 +1,4 @@
-"""Tile-loop microbenchmark (dev tool; GPU box): cycles per 8 KB tile per warp and bytes/clk per SM for the consumer side of
+"""Tile-loop microbenchmark (dev tool): cycles per 8 KB tile per warp and bytes/clk per SM for the consumer side of
 the decode kernel, by variant (bit 0: 128-bit LDS of fragment-ordered tiles instead of ldmatrix; bit 1: four accumulator
 chains instead of two; bit 2: no per-tile bookkeeping; bit 3: no mma). `python tools/tile_bench.py build` only compiles."""
 import ctypes as C, subprocess, sys
@@ -12,7 +12,7 @@ def build():
     src = ROOT / "csrc" / "tile_bench.cu"
     if LIB.exists() and LIB.stat().st_mtime > src.stat().st_mtime:
         return LIB
-    subprocess.run(["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    subprocess.run(["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
                     "-shared", "-Xcompiler", "-fPIC", "-o", str(LIB), str(src)], check=True)
     return LIB
 
@@ -26,7 +26,7 @@ if __name__ == "__main__":
     lib.dtk_dbg_tile_bench.restype = C.c_int
     lib.dtk_dbg_tile_bench.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     out = torch.zeros(4, device="cuda")
-    cyc = torch.zeros(148, dtype=torch.int64, device="cuda")
+    cyc = torch.zeros(132, dtype=torch.int64, device="cuda")
     s = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     iters, nslots = 4000, 24
     names = {0: "ldmatrix, 2 chains, bookkeeping (decode kernel today)", 1: "LDS.128 fragments, 2 chains, bookkeeping",
@@ -35,7 +35,7 @@ if __name__ == "__main__":
              8: "ldmatrix, NO mma, bookkeeping", 9: "LDS.128, NO mma, bookkeeping", 12: "ldmatrix, NO mma, no bookkeeping",
              13: "LDS.128, NO mma, no bookkeeping", 16: "TWO tiles interleaved per warp iteration, bookkeeping",
              20: "TWO tiles interleaved per warp iteration, no bookkeeping"}
-    for grid in (148,):
+    for grid in (132,):
         print(f"grid {grid}:")
         for v, nm in names.items():
             for _ in range(2):
