@@ -25,6 +25,16 @@ class DtkConfig(C.Structure):
     ]
 
 
+class DtkAdapterConfig(C.Structure):
+    _fields_ = [
+        ("hidden", C.c_int32), ("inter", C.c_int32), ("layers", C.c_int32), ("heads", C.c_int32),
+        ("kv_heads", C.c_int32), ("head_dim", C.c_int32), ("vocab", C.c_int32),
+        ("rms_eps", C.c_float), ("rope_theta", C.c_float), ("rope_factor", C.c_float),
+        ("rope_type", C.c_int32), ("rope_low_freq", C.c_float), ("rope_high_freq", C.c_float), ("rope_orig_max_pos", C.c_int32),
+        ("max_text", C.c_int32), ("cross_every_n", C.c_int32),
+    ]
+
+
 class DtkWeightInfo(C.Structure):
     _fields_ = [("name", C.c_char * 64), ("offset", C.c_uint64), ("nbytes", C.c_uint64),
                 ("rows", C.c_int32), ("cols", C.c_int32)]
@@ -48,6 +58,13 @@ SYMBOLS = {
     "dtk_last_error": (C.c_char_p, [_P]),
     "dtk_vit_encode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "dtk_project": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "dtk_adapter_weight_count": (C.c_int, [C.POINTER(DtkConfig), C.POINTER(DtkAdapterConfig)]),
+    "dtk_adapter_weight_get": (C.c_int, [C.POINTER(DtkConfig), C.POINTER(DtkAdapterConfig), C.c_int, C.POINTER(DtkWeightInfo)]),
+    "dtk_adapter_arena_bytes": (C.c_uint64, [C.POINTER(DtkConfig), C.POINTER(DtkAdapterConfig)]),
+    "dtk_adapter_attach": (C.c_int, [_P, C.POINTER(DtkAdapterConfig), _P, C.c_uint64]),
+    "dtk_adapter_detach": (C.c_int, [_P]),
+    "dtk_text_encode": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
+    "dtk_vit_encode_cond": (C.c_int, [_P, _P, C.c_int, _P, C.POINTER(C.c_int), C.c_int, _P, _P, _P]),
     "dtk_image_preprocess": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, C.c_int, C.c_float,
                                        C.POINTER(C.c_float), C.POINTER(C.c_float), _P, _P, _P, _P]),
     "dtk_seq_alloc": (C.c_int, [_P, C.POINTER(C.c_int)]),
@@ -74,6 +91,9 @@ SYMBOLS = {
     "dtk_dbg_flash_attn": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_float, _P]),
     "dtk_dbg_attn_tc": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P]),
+    "dtk_dbg_xattn_tc": (C.c_int, [_P, _P, C.POINTER(C.c_int), C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P]),
+    "dtk_dbg_head_layernorm": (C.c_int, [_P, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "dtk_dbg_gemm_gated": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "dtk_dbg_gemv": (C.c_int, [_P, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int, _P, _P]),
 }
 

@@ -2,6 +2,7 @@
 //   * ViT self-attention: 16 heads x head_dim 72 (zero-padded to 80 in shared memory for the
 //     QK^T contraction), N = 729 keys, non-causal  — HF modeling_siglip.py:229-249,293-306.
 //   * LLaMA prefill: head_dim 128, causal over cached positions — HF modeling_llama.py:199-222.
+//   * TikZero caption encoder (Llama-3.2-1B): head_dim 64, causal.
 // One CTA = 64 queries of one (batch, head); 4 warps x 16 query rows; K/V streamed in 64-key tiles
 // through a 2-stage cp.async ring. P is re-used straight from the score accumulators as the
 // A-operand of the PV product.
@@ -260,6 +261,7 @@ cudaError_t launch_flash_attn(const AttnArgs& a, cudaStream_t s, uint64_t* count
   if (counter) ++*counter;
   if (a.head_dim == 72) return a.causal ? launch_t<72, 80, true, false>(a, s) : launch_t<72, 80, false, false>(a, s);
   if (a.head_dim == 128) return a.causal ? launch_t<128, 128, true, false>(a, s) : launch_t<128, 128, false, false>(a, s);
+  if (a.head_dim == 64 && a.causal) return launch_t<64, 64, true, false>(a, s);   // caption encoder (Llama-3.2-1B)
   return cudaErrorInvalidValue;
 }
 

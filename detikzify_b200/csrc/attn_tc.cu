@@ -12,6 +12,9 @@
 //                              A operand of PV = P V (m64n80, K = 128: 8 wgmma, B = V^T tile), accumulated on top of the
 //                              rescaled fp32 output registers.
 // Keys past the image's 729 (rows of the next image / zero padding of V^T) are masked to -inf before the softmax.
+// The CROSS instantiation is the TikZero adapter's cross-attention (reference model/adapter/modeling_adapter.py:38-120): the
+// queries come from a [B*N, heads*72] matrix, the keys of image b are the first klen[b] rows of its Tk caption rows of a
+// [B*Tk, 2*heads*72] K | V matrix; keys at or past klen[b] are masked exactly like the padding keys above.
 // All mbarrier waits are bounded (trap instead of hanging the GPU).
 #include <cuda.h>
 
@@ -34,9 +37,13 @@ struct AttnTcArgs {
   int64_t o_rs;              // row stride (elements)
   int B, heads, N;           // tokens per image
   float scale_log2;          // scale * log2(e)
+  int kv_rows;               // CROSS: caption rows per image in the K map
+  int klen[XATTN_MAX_B];     // CROSS: valid keys of image b
 };
 
-__global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap mapQK,
+template <bool CROSS>
+__global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_constant__ CUtensorMap mapQ,
+                                                                 const __grid_constant__ CUtensorMap mapK,
                                                                  const __grid_constant__ CUtensorMap mapVT, const AttnTcArgs p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -47,7 +54,10 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_co
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * AQ;
-  const int nblk = (p.N + AK - 1) / AK;
+  const int nk = CROSS ? p.klen[b] : p.N;                   // keys of this image
+  const int krow0 = CROSS ? b * p.kv_rows : b * p.N;        // its first key row in the K map
+  const int khead = CROSS ? head : p.heads + head;          // K column block
+  const int nblk = (nk + AK - 1) / AK;
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -61,15 +71,15 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_co
     if (lane == 0) {
       const int row0 = b * p.N;
       mbar_expect_tx(q_full, 2 * QB);
-      tma_load_3d(sQ, &mapQK, 0, head, row0 + q0, q_full);                 // d 0..63
-      tma_load_3d(sQ + QB, &mapQK, 64, head, row0 + q0, q_full);           // d 64..127 (>= 72: zero fill)
+      tma_load_3d(sQ, &mapQ, 0, head, row0 + q0, q_full);                  // d 0..63
+      tma_load_3d(sQ + QB, &mapQ, 64, head, row0 + q0, q_full);            // d 64..127 (>= 72: zero fill)
       for (int j = 0; j < nblk; ++j) {
         const int s = j & 1, use = j >> 1;
         if (use > 0) mbar_wait(kv_empty0 + 8 * s, (use - 1) & 1);
         const uint32_t sk = sKV + s * KV_STAGE, sv = sk + 2 * QB;
         mbar_expect_tx(kv_full0 + 8 * s, KV_STAGE);
-        tma_load_3d(sk, &mapQK, 0, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
-        tma_load_3d(sk + QB, &mapQK, 64, p.heads + head, row0 + j * AK, kv_full0 + 8 * s);
+        tma_load_3d(sk, &mapK, 0, khead, krow0 + j * AK, kv_full0 + 8 * s);
+        tma_load_3d(sk + QB, &mapK, 64, khead, krow0 + j * AK, kv_full0 + 8 * s);
         tma_load_2d(sv, &mapVT, j * AK, (b * p.heads + head) * DP, kv_full0 + 8 * s);
         tma_load_2d(sv + VB, &mapVT, j * AK + 64, (b * p.heads + head) * DP, kv_full0 + 8 * s);
       }
@@ -96,7 +106,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 1) attn_tc_kernel(const __grid_co
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_acc_fence(sc);
-    const int kvalid = min(AK, p.N - j * AK);           // keys of this block that belong to the image
+    const int kvalid = min(AK, nk - j * AK);            // keys of this block that belong to the image
     float alpha[2], m_new[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {   // h = 0: row g, h = 1: row g + 8
@@ -181,6 +191,28 @@ __global__ void __launch_bounds__(256) transpose_v_kernel(const bf16* __restrict
   }
 }
 
+// V^T copy of the caption values: kv [B*Tk, 2*D] (v at column D + h*72 + d) -> vT [(b*heads + h)*80 + d, NP], zero for d >= 72
+// and for keys >= klen[b] (padded caption rows never reach the PV product). Same tiling as transpose_v_kernel.
+__global__ void __launch_bounds__(256) transpose_xv_kernel(const bf16* __restrict__ kv, int heads, int Tk, int D, int NP,
+                                                           const AttnTcArgs p, bf16* __restrict__ vT) {
+  __shared__ bf16 tile[32][33];
+  const int bh = blockIdx.z, b = bh / heads, h = bh % heads;
+  const int k0 = blockIdx.x * 32, d0 = blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int nk = p.klen[b];
+  for (int i = ty; i < 32; i += 8) {
+    const int key = k0 + i, d = d0 + tx;
+    bf16 v = __float2bfloat16_rn(0.f);
+    if (key < nk && d < DH) v = kv[(int64_t)(b * Tk + key) * (2 * D) + D + h * DH + d];
+    tile[i][tx] = v;
+  }
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8) {
+    const int d = d0 + i, key = k0 + tx;
+    if (d < DP && key < NP) vT[((int64_t)bh * DP + d) * NP + key] = tile[tx][i];
+  }
+}
+
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -197,6 +229,41 @@ EncodeFn a_encode_fn() {
   return fn;
 }
 
+// rank-3 view [rows][cols / 72][72] of a bf16 matrix with row stride ld: box 64 (d) x 1 (head) x 128 (rows), 128-byte swizzle,
+// zero fill past d = 72
+bool map_heads(EncodeFn fn, CUtensorMap* map, const bf16* ptr, int64_t rows, int col_heads, int64_t ld) {
+  cuuint64_t dims[3] = {(cuuint64_t)DH, (cuuint64_t)col_heads, (cuuint64_t)rows};
+  cuuint64_t strides[2] = {(cuuint64_t)DH * 2, (cuuint64_t)ld * 2};
+  cuuint32_t box[3] = {64, 1, (cuuint32_t)AQ};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// V^T [rows, NP]: box 64 keys x 80 rows
+bool map_vt(EncodeFn fn, CUtensorMap* map, const bf16* vT, int64_t rows, int NP) {
+  cuuint64_t dims[2] = {(cuuint64_t)NP, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)NP * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)DP};
+  cuuint32_t estr[2] = {1, 1};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)vT, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <bool CROSS>
+cudaError_t set_smem_attr() {
+  static bool attr_done[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64 || !attr_done[dev]) {
+    e = cudaFuncSetAttribute(attn_tc_kernel<CROSS>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATC_SMEM);
+    if (e != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) attr_done[dev] = true;
+  }
+  return cudaSuccess;
+}
+
 }  // namespace
 
 bool attn_tc_supported() { return a_encode_fn() != nullptr; }
@@ -208,36 +275,39 @@ cudaError_t launch_attn_tc(const bf16* qkv, bf16* vT, bf16* o, int B, int heads,
   if (!fn) return cudaErrorNotSupported;
   const int D = heads * DH, NP = attn_tc_vt_cols(N);
   CUtensorMap mapQK, mapVT;
-  {  // qkv viewed as [token][3*heads][72]: box 64 (d) x 1 (head) x 128 (tokens), 128-byte swizzle, zero fill past d = 72
-    cuuint64_t dims[3] = {(cuuint64_t)DH, (cuuint64_t)(3 * heads), (cuuint64_t)B * N};
-    cuuint64_t strides[2] = {(cuuint64_t)DH * 2, (cuuint64_t)3 * D * 2};
-    cuuint32_t box[3] = {64, 1, (cuuint32_t)AQ};
-    cuuint32_t estr[3] = {1, 1, 1};
-    if (fn(&mapQK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)qkv, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cudaErrorInvalidValue;
-  }
-  {  // V^T [B*heads*80, NP]: box 64 keys x 80 rows
-    cuuint64_t dims[2] = {(cuuint64_t)NP, (cuuint64_t)B * heads * DP};
-    cuuint64_t strides[1] = {(cuuint64_t)NP * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)DP};
-    cuuint32_t estr[2] = {1, 1};
-    if (fn(&mapVT, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)vT, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cudaErrorInvalidValue;
-  }
-  static bool attr_done[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  // qkv viewed as [token][3*heads][72]
+  if (!map_heads(fn, &mapQK, qkv, (int64_t)B * N, 3 * heads, 3 * D) || !map_vt(fn, &mapVT, vT, (int64_t)B * heads * DP, NP))
+    return cudaErrorInvalidValue;
+  cudaError_t e = set_smem_attr<false>();
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-    e = cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATC_SMEM);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) attr_done[dev] = true;
-  }
   transpose_v_kernel<<<dim3(NP / 32, 3, B * heads), 256, 0, s>>>(qkv, B, heads, N, D, NP, vT);
-  AttnTcArgs a{o, (int64_t)D, B, heads, N, scale * 1.4426950408889634f};
-  attn_tc_kernel<<<dim3((N + AQ - 1) / AQ, heads, B), ATC_THREADS, ATC_SMEM, s>>>(mapQK, mapVT, a);
+  AttnTcArgs a{};
+  a.o = o; a.o_rs = D; a.B = B; a.heads = heads; a.N = N; a.scale_log2 = scale * 1.4426950408889634f;
+  attn_tc_kernel<false><<<dim3((N + AQ - 1) / AQ, heads, B), ATC_THREADS, ATC_SMEM, s>>>(mapQK, mapQK, mapVT, a);
+  if (counter) *counter += 2;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_xattn_tc(const bf16* q, const bf16* kv, const int* klen_host, int Tk, bf16* vT, bf16* o, int B, int heads,
+                            int N, float scale, cudaStream_t s, uint64_t* counter) {
+  EncodeFn fn = a_encode_fn();
+  if (!fn) return cudaErrorNotSupported;
+  if (B <= 0 || B > XATTN_MAX_B || Tk <= 0 || N <= 0 || heads <= 0) return cudaErrorInvalidValue;
+  AttnTcArgs a{};
+  for (int b = 0; b < B; ++b) {
+    if (klen_host[b] < 1 || klen_host[b] > Tk) return cudaErrorInvalidValue;
+    a.klen[b] = klen_host[b];
+  }
+  const int D = heads * DH, NP = attn_tc_vt_cols(Tk);
+  CUtensorMap mapQ, mapK, mapVT;
+  if (!map_heads(fn, &mapQ, q, (int64_t)B * N, heads, D) || !map_heads(fn, &mapK, kv, (int64_t)B * Tk, 2 * heads, 2 * D) ||
+      !map_vt(fn, &mapVT, vT, (int64_t)B * heads * DP, NP))
+    return cudaErrorInvalidValue;
+  cudaError_t e = set_smem_attr<true>();
+  if (e != cudaSuccess) return e;
+  a.o = o; a.o_rs = D; a.B = B; a.heads = heads; a.N = N; a.scale_log2 = scale * 1.4426950408889634f; a.kv_rows = Tk;
+  transpose_xv_kernel<<<dim3(NP / 32, 3, B * heads), 256, 0, s>>>(kv, heads, Tk, D, NP, a, vT);
+  attn_tc_kernel<true><<<dim3((N + AQ - 1) / AQ, heads, B), ATC_THREADS, ATC_SMEM, s>>>(mapQ, mapK, mapVT, a);
   if (counter) *counter += 2;
   return cudaGetLastError();
 }

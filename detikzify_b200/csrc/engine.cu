@@ -95,6 +95,91 @@ bool config_ok(const dtk_config& c, std::string& why) {
   return true;
 }
 
+// TikZero adapter arena: caption embedder (LlamaModel without lm_head), connector, one cross layer per selected vision layer
+// (reference model/adapter/modeling_adapter.py:293-394), dummy image
+bool has_cross(const dtk_adapter_config& a, int l) { return (l + 1) % a.cross_every_n == 0; }
+
+std::vector<WEntry> build_adapter_table(const dtk_config& c, const dtk_adapter_config& a) {
+  std::vector<WEntry> t;
+  uint64_t off = 0;
+  auto add = [&](const std::string& n, int rows, int cols) {
+    WEntry e{n, rows, cols, off, (uint64_t)rows * cols * 2};
+    off = align_up(off + e.nbytes, 256);
+    t.push_back(e);
+  };
+  const int E = a.hidden, I = a.inter, qd = a.heads * 64, kd = a.kv_heads * 64;
+  add("emb.embed", a.vocab, E);
+  for (int l = 0; l < a.layers; ++l) {
+    std::string p = "emb.L" + std::to_string(l) + ".";
+    add(p + "norm1", 1, E);
+    add(p + "wqkv", qd + 2 * kd, E);
+    add(p + "wo", E, qd);
+    add(p + "norm2", 1, E);
+    add(p + "wgu", 2 * I, E);  // interleaved rows: 2i = gate_i, 2i+1 = up_i
+    add(p + "wd", E, I);
+  }
+  add("emb.norm", 1, E);
+  const int D = c.v_hidden, VI = c.v_inter;
+  add("ad.connector_w", D, E); add("ad.connector_b", 1, D);
+  for (int l = 0; l < c.v_layers; ++l) {
+    if (!has_cross(a, l)) continue;
+    std::string p = "ad.L" + std::to_string(l) + ".";
+    add(p + "ln1_w", 1, D); add(p + "ln1_b", 1, D);
+    add(p + "wq", D, D); add(p + "bq", 1, D);
+    add(p + "wkv", 2 * D, D); add(p + "bkv", 1, 2 * D);
+    add(p + "wo", D, D); add(p + "bo", 1, D);
+    add(p + "q_norm_w", 1, 72); add(p + "q_norm_b", 1, 72);
+    add(p + "k_norm_w", 1, 72); add(p + "k_norm_b", 1, 72);
+    add(p + "ln2_w", 1, D); add(p + "ln2_b", 1, D);
+    add(p + "w1", VI, D); add(p + "b1", 1, VI);
+    add(p + "w2", D, VI); add(p + "b2", 1, D);
+    add(p + "attn_gate", 1, 1); add(p + "mlp_gate", 1, 1);
+  }
+  add("ad.dummy", 3, c.v_image * c.v_image);
+  return t;
+}
+
+bool adapter_config_ok(const dtk_config& c, const dtk_adapter_config& a, std::string& why) {
+  auto bad = [&](const char* m) { why = m; return false; };
+  if (!config_ok(c, why)) return false;
+  if (a.hidden <= 0 || a.inter <= 0 || a.layers <= 0 || a.heads <= 0 || a.kv_heads <= 0 || a.vocab <= 0) return bad("non-positive embedder dims");
+  if (a.head_dim != 64) return bad("embedder head_dim must be 64");
+  if (a.heads % a.kv_heads) return bad("embedder heads % kv_heads != 0");
+  if ((a.hidden & 7) || (a.inter & 7)) return bad("embedder hidden/inter must be multiples of 8");
+  if (a.rope_type != 0 && a.rope_type != 1) return bad("rope_type must be 0 (linear) or 1 (llama3)");
+  if (a.rope_type == 1 && (a.rope_low_freq <= 0.f || a.rope_high_freq <= a.rope_low_freq || a.rope_orig_max_pos <= 0)) return bad("bad llama3 rope parameters");
+  if (a.max_text <= 0 || a.max_text > 8192) return bad("max_text must be in 1..8192");
+  if (a.cross_every_n <= 0) return bad("cross_every_n must be positive");
+  return true;
+}
+
+// RoPE cos/sin table [T, hd/2, 2] (HF modeling_llama.py:83-121: inv_freq = theta^(-2i/d) / factor, fp32; angle = pos * inv_freq)
+std::vector<float> rope_table(float theta, float factor, int type, float low_freq, float high_freq, int orig_max_pos, int hd, int64_t T) {
+  const int half = hd / 2;
+  std::vector<float> tab((size_t)T * half * 2);
+  for (int i = 0; i < half; ++i) {
+    float inv = 1.0f / powf(theta, (float)(2 * i) / (float)hd);
+    if (type == 1) {   // llama3 (HF modeling_rope_utils.py _compute_llama3_parameters), fp32 like HF
+      const float old_len = (float)orig_max_pos;
+      const float low_wl = old_len / low_freq, high_wl = old_len / high_freq;
+      const float wl = 2.0f * 3.14159265358979323846f / inv;
+      if (wl > low_wl) inv = inv / factor;
+      else if (!(wl < high_wl)) {
+        const float smooth = (old_len / wl - low_freq) / (high_freq - low_freq);
+        inv = (1.0f - smooth) * inv / factor + smooth * inv;
+      }
+    } else {
+      inv = inv / factor;
+    }
+    for (int64_t p = 0; p < T; ++p) {
+      float ang = (float)p * inv;
+      tab[((size_t)p * half + i) * 2] = (float)cos((double)ang);
+      tab[((size_t)p * half + i) * 2 + 1] = (float)sin((double)ang);
+    }
+  }
+  return tab;
+}
+
 }  // namespace
 
 struct dtk_engine {
@@ -171,6 +256,15 @@ struct dtk_engine {
   int fuse_greedy = 1;
   int cascade_attn = 1;      // batched decode: rows that share one prefix reduce it with ONE tensor-core pass (option "cascade_attn")
   int cas_slot = -1, cas_len = 0;   // set per step by dtk_decode / dtk_gen_begin: uniform shared prefix of the current batch
+
+  // TikZero adapter (dtk_adapter_attach): borrowed arena, caption-encoder workspace (max_text rows) and the conditioned
+  // ViT's caption buffers (one ViT chunk of captions)
+  bool has_adapter = false;
+  dtk_adapter_config acfg{};
+  std::map<std::string, const bf16*> aw;
+  float *t_rope = nullptr, *t_x = nullptr, *t_qkv = nullptr;
+  bf16 *t_xn = nullptr, *t_q = nullptr, *t_k = nullptr, *t_v = nullptr, *t_att = nullptr, *t_h = nullptr;
+  bf16 *x_cond = nullptr, *x_kv = nullptr, *x_vt = nullptr;
 };
 
 namespace {
@@ -285,8 +379,65 @@ int ensure_probe_query(dtk_engine* eng, cudaStream_t s) {
   return DTK_OK;
 }
 
-// ViT blocks for B images already resident as fp32 pixels; leaves post-LN tokens (bf16) in v_xn.
-int vit_forward(dtk_engine* eng, const float* pixels, int B, float* tokens_out, float* pooled_out, cudaStream_t s) {
+// caption conditioning of one ViT chunk: bf16 caption states [B, Tmax, D] (rows >= len[b] of caption b are padding)
+struct XCond {
+  const bf16* cond;
+  const int* len;   // host int[B]
+  int Tmax;
+};
+
+// TikZero cross layer l on the residual stream v_x (reference modeling_adapter.py:326-352, run as a forward pre-hook of vision
+// layer l): x += sigmoid(g_attn) * out_proj(xattn(q_norm(q_proj(LN1 x)), k_norm(k_proj(cond)), v_proj(cond)));
+// x += sigmoid(g_mlp) * fc2(act(fc1(LN2 x)))
+int cross_layer(dtk_engine* eng, int l, const XCond& xc, int B, cudaStream_t s) {
+  const dtk_config& c = eng->cfg;
+  const int D = c.v_hidden, VI = c.v_inter, N = v_tokens(c), M = B * N, Mk = B * xc.Tmax;
+  const int act = c.v_act == 1 ? ACT_GELU_ERF : ACT_GELU_TANH;
+  uint64_t* lc = &eng->launches;
+  auto aw = [&](const char* n) { return eng->aw.at(LN("ad.L", l, n)); };
+  DTK_CK(launch_layernorm(eng->v_x, aw("ln1_w"), aw("ln1_b"), c.v_eps, M, D, eng->v_xn, nullptr, s, lc));
+  bf16* q = eng->v_qkv;   // [M, D]
+  {
+    GemmArgs g{};
+    g.A = eng->v_xn; g.lda = D; g.W = aw("wq"); g.ldw = D; g.M = M; g.N = D; g.K = D;
+    g.bias = aw("bq"); g.out_bf16 = q; g.ldo = D;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  DTK_CK(launch_head_layernorm(q, D, aw("q_norm_w"), aw("q_norm_b"), c.v_eps, M, c.v_heads, 72, q, D, s, lc));
+  {  // K | V of the captions, once per layer for the whole chunk
+    GemmArgs g{};
+    g.A = xc.cond; g.lda = D; g.W = aw("wkv"); g.ldw = D; g.M = Mk; g.N = 2 * D; g.K = D;
+    g.bias = aw("bkv"); g.out_bf16 = eng->x_kv; g.ldo = 2 * D;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  DTK_CK(launch_head_layernorm(eng->x_kv, 2 * D, aw("k_norm_w"), aw("k_norm_b"), c.v_eps, Mk, c.v_heads, 72, eng->x_kv, 2 * D, s, lc));
+  DTK_CK(launch_xattn_tc(q, eng->x_kv, xc.len, xc.Tmax, eng->x_vt, eng->v_att, B, c.v_heads, N, 1.0f / sqrtf(72.f), s, lc));
+  {
+    GemmArgs g{};
+    g.A = eng->v_att; g.lda = D; g.W = aw("wo"); g.ldw = D; g.M = M; g.N = D; g.K = D;
+    g.bias = aw("bo"); g.gate = aw("attn_gate"); g.resid = eng->v_x; g.ldr = D; g.out_f32 = eng->v_x; g.ldo = D;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  DTK_CK(launch_layernorm(eng->v_x, aw("ln2_w"), aw("ln2_b"), c.v_eps, M, D, eng->v_xn, nullptr, s, lc));
+  {
+    GemmArgs g{};
+    g.A = eng->v_xn; g.lda = D; g.W = aw("w1"); g.ldw = D; g.M = M; g.N = VI; g.K = D;
+    g.bias = aw("b1"); g.act = act; g.out_bf16 = eng->v_h; g.ldo = VI;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  {
+    GemmArgs g{};
+    g.A = eng->v_h; g.lda = VI; g.W = aw("w2"); g.ldw = VI; g.M = M; g.N = D; g.K = VI;
+    g.bias = aw("b2"); g.gate = aw("mlp_gate"); g.resid = eng->v_x; g.ldr = D; g.out_f32 = eng->v_x; g.ldo = D;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  return DTK_OK;
+}
+
+// ViT blocks for B images already resident as fp32 pixels; leaves post-LN tokens (bf16) in v_xn. xc (TikZero) inserts the
+// adapter's cross layers before the vision layers that have one.
+int vit_forward(dtk_engine* eng, const float* pixels, int B, float* tokens_out, float* pooled_out, cudaStream_t s,
+                const XCond* xc = nullptr) {
   const dtk_config& c = eng->cfg;
   const int D = c.v_hidden, VI = c.v_inter, N = v_tokens(c), KP = patch_k_padded(c);
   const int M = B * N;
@@ -302,6 +453,10 @@ int vit_forward(dtk_engine* eng, const float* pixels, int B, float* tokens_out, 
     DTK_CK(launch_gemm(g, s, lc));
   }
   for (int l = 0; l < c.v_layers; ++l) {
+    if (xc && has_cross(eng->acfg, l)) {
+      int r = cross_layer(eng, l, *xc, B, s);
+      if (r != DTK_OK) return r;
+    }
     DTK_CK(launch_layernorm(eng->v_x, W(eng, LN("vit.L", l, "ln1_w")), W(eng, LN("vit.L", l, "ln1_b")), c.v_eps, M, D, eng->v_xn, nullptr, s, lc));
     {
       GemmArgs g{};
@@ -618,29 +773,9 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
   eng->refcnt.assign(c.max_seqs, 0);
   eng->shared_upto.assign(c.max_seqs, 0);
 
-  // RoPE table (HF modeling_llama.py:83-121: inv_freq = theta^(-2i/d) / factor, fp32; angle = pos * inv_freq)
   {
-    std::vector<float> tab((size_t)T * 64 * 2);
-    for (int i = 0; i < 64; ++i) {
-      float inv = 1.0f / powf(c.rope_theta, (float)(2 * i) / 128.0f);
-      if (c.rope_type == 1) {   // llama3 (HF modeling_rope_utils.py _compute_llama3_parameters), fp32 like HF
-        const float old_len = (float)c.rope_orig_max_pos;
-        const float low_wl = old_len / c.rope_low_freq, high_wl = old_len / c.rope_high_freq;
-        const float wl = 2.0f * 3.14159265358979323846f / inv;
-        if (wl > low_wl) inv = inv / c.rope_factor;
-        else if (!(wl < high_wl)) {
-          const float smooth = (old_len / wl - c.rope_low_freq) / (c.rope_high_freq - c.rope_low_freq);
-          inv = (1.0f - smooth) * inv / c.rope_factor + smooth * inv;
-        }
-      } else {
-        inv = inv / c.rope_factor;
-      }
-      for (int64_t p = 0; p < T; ++p) {
-        float ang = (float)p * inv;
-        tab[((size_t)p * 64 + i) * 2] = (float)cos((double)ang);
-        tab[((size_t)p * 64 + i) * 2 + 1] = (float)sin((double)ang);
-      }
-    }
+    std::vector<float> tab = rope_table(c.rope_theta, c.rope_factor, c.rope_type, c.rope_low_freq, c.rope_high_freq,
+                                        c.rope_orig_max_pos, 128, T);
     DTK_ALLOC(eng->rope_cs, tab.size());
     DTK_CK(cudaMemcpy(eng->rope_cs, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
@@ -753,6 +888,7 @@ int dtk_destroy(dtk_engine* eng) {
                   eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
                   eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b};
   for (void* p : ptrs) if (p) cudaFree(p);
+  dtk_adapter_detach(eng);
   if (eng->cap_stream) cudaStreamDestroy(eng->cap_stream);
   if (eng->host_ring) cudaFreeHost(eng->host_ring);
   cudaGetLastError();
@@ -806,6 +942,171 @@ int dtk_vit_encode(dtk_engine* eng, const float* pixels, int B, float* tokens_ou
     eng->launches += it->second.launches;
     if (tok) DTK_CK(cudaMemcpyAsync(tok, eng->v_tok_out, (size_t)nb * N * D * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (pool) DTK_CK(cudaMemcpyAsync(pool, eng->v_pool_out, (size_t)nb * D * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  }
+  return DTK_OK;
+}
+
+int dtk_adapter_weight_count(const dtk_config* cfg, const dtk_adapter_config* acfg) {
+  if (!cfg || !acfg) return DTK_ERR_INVALID;
+  std::string why;
+  if (!adapter_config_ok(*cfg, *acfg, why)) return DTK_ERR_INVALID;
+  return (int)build_adapter_table(*cfg, *acfg).size();
+}
+
+int dtk_adapter_weight_get(const dtk_config* cfg, const dtk_adapter_config* acfg, int index, dtk_weight_info* out) {
+  if (!cfg || !acfg || !out) return DTK_ERR_INVALID;
+  std::string why;
+  if (!adapter_config_ok(*cfg, *acfg, why)) return DTK_ERR_INVALID;
+  auto t = build_adapter_table(*cfg, *acfg);
+  if (index < 0 || index >= (int)t.size()) return DTK_ERR_INVALID;
+  std::memset(out, 0, sizeof(*out));
+  std::snprintf(out->name, sizeof(out->name), "%s", t[index].name.c_str());
+  out->offset = t[index].offset; out->nbytes = t[index].nbytes; out->rows = t[index].rows; out->cols = t[index].cols;
+  return DTK_OK;
+}
+
+uint64_t dtk_adapter_arena_bytes(const dtk_config* cfg, const dtk_adapter_config* acfg) {
+  if (!cfg || !acfg) return 0;
+  std::string why;
+  if (!adapter_config_ok(*cfg, *acfg, why)) return 0;
+  auto t = build_adapter_table(*cfg, *acfg);
+  return align_up(t.back().offset + t.back().nbytes, 256);
+}
+
+int dtk_adapter_detach(dtk_engine* eng) {
+  if (!eng) return DTK_ERR_INVALID;
+  cudaSetDevice(eng->device);
+  cudaDeviceSynchronize();   // buffers may still be read by queued work
+  void* ptrs[] = {eng->t_rope, eng->t_x, eng->t_qkv, eng->t_xn, eng->t_q, eng->t_k, eng->t_v, eng->t_att, eng->t_h,
+                  eng->x_cond, eng->x_kv, eng->x_vt};
+  for (void* p : ptrs) if (p) cudaFree(p);
+  eng->t_rope = eng->t_x = eng->t_qkv = nullptr;
+  eng->t_xn = eng->t_q = eng->t_k = eng->t_v = eng->t_att = eng->t_h = nullptr;
+  eng->x_cond = eng->x_kv = eng->x_vt = nullptr;
+  eng->aw.clear();
+  eng->has_adapter = false;
+  return DTK_OK;
+}
+
+int dtk_adapter_attach(dtk_engine* eng, const dtk_adapter_config* acfg, const void* arena, uint64_t arena_bytes) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(acfg && arena, "null pointer");
+  std::string why;
+  if (!adapter_config_ok(eng->cfg, *acfg, why)) { eng->err = "invalid adapter config: " + why; return DTK_ERR_INVALID; }
+  DTK_REQUIRE(arena_bytes >= dtk_adapter_arena_bytes(&eng->cfg, acfg), "adapter arena too small");
+  dtk_adapter_detach(eng);
+  DTK_CK(cudaSetDevice(eng->device));
+  eng->acfg = *acfg;
+  for (auto& e : build_adapter_table(eng->cfg, *acfg)) eng->aw[e.name] = (const bf16*)((const uint8_t*)arena + e.offset);
+  const dtk_adapter_config& a = eng->acfg;
+  const dtk_config& c = eng->cfg;
+  const int64_t T = a.max_text, E = a.hidden, qd = a.heads * 64, kd = a.kv_heads * 64;
+  {
+    std::vector<float> tab = rope_table(a.rope_theta, a.rope_factor, a.rope_type, a.rope_low_freq, a.rope_high_freq,
+                                        a.rope_orig_max_pos, 64, T);
+    DTK_ALLOC(eng->t_rope, tab.size());
+    DTK_CK(cudaMemcpy(eng->t_rope, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  DTK_ALLOC(eng->t_x, T * E);
+  DTK_ALLOC(eng->t_qkv, T * (qd + 2 * kd));
+  DTK_ALLOC(eng->t_xn, T * E);
+  DTK_ALLOC(eng->t_q, T * qd);
+  DTK_ALLOC(eng->t_k, T * kd);
+  DTK_ALLOC(eng->t_v, T * kd);
+  DTK_ALLOC(eng->t_att, T * qd);
+  DTK_ALLOC(eng->t_h, T * a.inter);
+  const int64_t crow = (int64_t)VIT_CHUNK * T;
+  DTK_ALLOC(eng->x_cond, crow * c.v_hidden);
+  DTK_ALLOC(eng->x_kv, crow * 2 * c.v_hidden);
+  DTK_ALLOC(eng->x_vt, (int64_t)VIT_CHUNK * c.v_heads * 80 * attn_tc_vt_cols((int)T));
+  eng->has_adapter = true;
+  return DTK_OK;
+}
+
+int dtk_text_encode(dtk_engine* eng, const int64_t* ids, int T, float* hidden_out, float* cond_out, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->has_adapter, "no adapter attached");
+  DTK_REQUIRE(ids && cond_out, "null pointer");
+  const dtk_adapter_config& a = eng->acfg;
+  DTK_REQUIRE(T >= 1 && T <= a.max_text, "T must be in 1..max_text");
+  DTK_CK(cudaSetDevice(eng->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  uint64_t* lc = &eng->launches;
+  const int E = a.hidden, I = a.inter, qd = a.heads * 64, kd = a.kv_heads * 64, qkvd = qd + 2 * kd;
+  auto aw = [&](const std::string& n) { return eng->aw.at(n); };
+  DTK_CK(launch_embed_splice(ids, T, 0, aw("emb.embed"), E, a.vocab, -1, nullptr, 0, 0, eng->t_x, s, lc));
+  for (int l = 0; l < a.layers; ++l) {
+    DTK_CK(launch_rmsnorm(eng->t_x, E, aw(LN("emb.L", l, "norm1")), a.rms_eps, T, E, eng->t_xn, s, lc));
+    {
+      GemmArgs g{};
+      g.A = eng->t_xn; g.lda = E; g.W = aw(LN("emb.L", l, "wqkv")); g.ldw = E; g.M = T; g.N = qkvd; g.K = E;
+      g.out_f32 = eng->t_qkv; g.ldo = qkvd;
+      DTK_CK(launch_gemm(g, s, lc));
+    }
+    DTK_CK(launch_rope_qkv64(eng->t_qkv, T, a.heads, a.kv_heads, eng->t_rope, eng->t_q, eng->t_k, eng->t_v, s, lc));
+    {
+      AttnArgs f{};
+      f.q = eng->t_q; f.k = eng->t_k; f.v = eng->t_v; f.o = eng->t_att;
+      f.q_bs = 0; f.q_hs = 64; f.q_rs = qd;
+      f.k_bs = 0; f.k_hs = 64; f.k_rs = kd;
+      f.v_bs = 0; f.v_hs = 64; f.v_rs = kd;
+      f.o_bs = 0; f.o_hs = 64; f.o_rs = qd;
+      f.B = 1; f.heads = a.heads; f.kv_group = a.heads / a.kv_heads; f.Tq = T; f.Tk = T; f.q_pos0 = 0;
+      f.causal = 1; f.head_dim = 64; f.scale = 0.125f;
+      DTK_CK(launch_flash_attn(f, s, lc));
+    }
+    {
+      GemmArgs g{};
+      g.A = eng->t_att; g.lda = qd; g.W = aw(LN("emb.L", l, "wo")); g.ldw = qd; g.M = T; g.N = E; g.K = qd;
+      g.resid = eng->t_x; g.ldr = E; g.out_f32 = eng->t_x; g.ldo = E;
+      DTK_CK(launch_gemm(g, s, lc));
+    }
+    DTK_CK(launch_rmsnorm(eng->t_x, E, aw(LN("emb.L", l, "norm2")), a.rms_eps, T, E, eng->t_xn, s, lc));
+    {
+      GemmArgs g{};
+      g.A = eng->t_xn; g.lda = E; g.W = aw(LN("emb.L", l, "wgu")); g.ldw = E; g.M = T; g.N = 2 * I; g.K = E;
+      g.glu = 1; g.out_bf16 = eng->t_h; g.ldo = I;
+      DTK_CK(launch_gemm(g, s, lc));
+    }
+    {
+      GemmArgs g{};
+      g.A = eng->t_h; g.lda = I; g.W = aw(LN("emb.L", l, "wd")); g.ldw = I; g.M = T; g.N = E; g.K = I;
+      g.resid = eng->t_x; g.ldr = E; g.out_f32 = eng->t_x; g.ldo = E;
+      DTK_CK(launch_gemm(g, s, lc));
+    }
+  }
+  DTK_CK(launch_rmsnorm(eng->t_x, E, aw("emb.norm"), a.rms_eps, T, E, eng->t_xn, s, lc));
+  if (hidden_out) DTK_CK(launch_cast_bf16_f32(eng->t_xn, hidden_out, (int64_t)T * E, s, lc));
+  {
+    GemmArgs g{};
+    g.A = eng->t_xn; g.lda = E; g.W = aw("ad.connector_w"); g.ldw = E; g.M = T; g.N = eng->cfg.v_hidden; g.K = E;
+    g.bias = aw("ad.connector_b"); g.out_f32 = cond_out; g.ldo = eng->cfg.v_hidden;
+    DTK_CK(launch_gemm(g, s, lc));
+  }
+  return DTK_OK;
+}
+
+int dtk_vit_encode_cond(dtk_engine* eng, const float* pixels, int B, const float* cond, const int* cond_len, int Tmax,
+                        float* tokens_out, float* pooled_out, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->has_adapter, "no adapter attached");
+  DTK_REQUIRE(pixels && cond && cond_len && B > 0, "pixels/cond/cond_len/B");
+  DTK_REQUIRE(Tmax >= 1 && Tmax <= eng->acfg.max_text, "Tmax must be in 1..max_text");
+  for (int b = 0; b < B; ++b) DTK_REQUIRE(cond_len[b] >= 1 && cond_len[b] <= Tmax, "cond_len[b] must be in 1..Tmax");
+  DTK_CK(cudaSetDevice(eng->device));
+  const dtk_config& c = eng->cfg;
+  cudaStream_t s = (cudaStream_t)stream;
+  int r = ensure_vit_ws(eng, B);
+  if (r != DTK_OK) return r;
+  if (pooled_out && (r = ensure_probe_query(eng, s)) != DTK_OK) return r;
+  const int64_t pix_per = (int64_t)3 * c.v_image * c.v_image, N = v_tokens(c), D = c.v_hidden;
+  for (int b0 = 0; b0 < B; b0 += VIT_CHUNK) {
+    const int nb = B - b0 < VIT_CHUNK ? B - b0 : VIT_CHUNK;
+    DTK_CK(launch_cast_f32_bf16(cond + (int64_t)b0 * Tmax * D, eng->x_cond, (int64_t)nb * Tmax * D, s, &eng->launches));
+    XCond xc{eng->x_cond, cond_len + b0, Tmax};
+    r = vit_forward(eng, pixels + b0 * pix_per, nb, tokens_out ? tokens_out + b0 * N * D : nullptr,
+                    pooled_out ? pooled_out + (int64_t)b0 * D : nullptr, s, &xc);
+    if (r != DTK_OK) return r;
   }
   return DTK_OK;
 }
@@ -1335,6 +1636,32 @@ int dtk_dbg_attn_tc(const void* qkv, void* vt_scratch, void* o, int B, int heads
   if (!qkv || !vt_scratch || !o || B <= 0 || heads <= 0 || N <= 0) return DTK_ERR_INVALID;
   if (!attn_tc_supported()) return DTK_ERR_UNSUPPORTED;
   return launch_attn_tc((const bf16*)qkv, (bf16*)vt_scratch, (bf16*)o, B, heads, N, scale, (cudaStream_t)stream, nullptr) == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
+}
+
+int dtk_dbg_xattn_tc(const void* q, const void* kv, const int* klen_host, int Tk, void* vt_scratch, void* o, int B, int heads,
+                     int N, float scale, void* stream) {
+  if (!q || !kv || !klen_host || !vt_scratch || !o || B <= 0 || B > XATTN_MAX_B || heads <= 0 || N <= 0 || Tk <= 0) return DTK_ERR_INVALID;
+  for (int b = 0; b < B; ++b) if (klen_host[b] < 1 || klen_host[b] > Tk) return DTK_ERR_INVALID;
+  if (!attn_tc_supported()) return DTK_ERR_UNSUPPORTED;
+  return launch_xattn_tc((const bf16*)q, (const bf16*)kv, klen_host, Tk, (bf16*)vt_scratch, (bf16*)o, B, heads, N, scale,
+                         (cudaStream_t)stream, nullptr) == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
+}
+
+int dtk_dbg_head_layernorm(const void* x, const void* w, const void* b, float eps, int M, int heads, int hd, void* out, void* stream) {
+  if (!x || !w || !b || !out || M <= 0 || heads <= 0) return DTK_ERR_INVALID;
+  const int64_t ld = (int64_t)heads * hd;
+  return launch_head_layernorm((const bf16*)x, ld, (const bf16*)w, (const bf16*)b, eps, M, heads, hd, (bf16*)out, ld,
+                               (cudaStream_t)stream, nullptr) == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
+}
+
+int dtk_dbg_gemm_gated(const void* A, const void* Wm, const void* bias, const void* gate, const float* resid, int M, int N, int K,
+                       int act, float* out_f32, void* stream) {
+  if (!A || !Wm || !gate || !out_f32) return DTK_ERR_INVALID;
+  GemmArgs g{};
+  g.A = (const bf16*)A; g.lda = K; g.W = (const bf16*)Wm; g.ldw = K; g.M = M; g.N = N; g.K = K;
+  g.bias = (const bf16*)bias; g.gate = (const bf16*)gate; g.resid = resid; g.ldr = N; g.act = act;
+  g.out_f32 = out_f32; g.ldo = N;
+  return launch_gemm(g, (cudaStream_t)stream, nullptr) == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
 }
 
 int dtk_dbg_gemv(const void* Wm, const float* x, const void* norm_w, float eps, int N, int K, int mode, float* out,

@@ -138,6 +138,10 @@ __global__ void __launch_bounds__(THREADS) gemm_bf16_tn_kernel(const GemmArgs p)
           else p.out_f32[o] = r;
           continue;
         }
+        if (p.gate) {
+          const float gs = 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
+          v0 *= gs; v1 *= gs;
+        }
         if (p.rowbias) {
           float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rowbias + (int64_t)(m % p.rowbias_mod) * p.N + n));
           v0 += b.x; v1 += b.y;
@@ -161,6 +165,7 @@ void set_gemm_impl(int impl) { g_gemm_impl = impl; }
 int get_gemm_impl() { return g_gemm_impl; }
 
 cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
+  if (a.gate && a.glu) return cudaErrorInvalidValue;   // the GLU epilogue has no gate
   // large-M dense contractions go to the wgmma kernel; tiny M (pool head, M = B) stays on mma.sync
   // (M < 4: pool-head probes and other tiny products stay on mma.sync; 4 <= M < 64 takes the swapped-operand wgmma tile)
   if (g_gemm_impl >= 1 && a.M >= 4 && gemm_tc_supported(a)) return launch_gemm_tc(a, s, counter);

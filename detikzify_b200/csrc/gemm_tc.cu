@@ -58,6 +58,10 @@ DTK_DEV void dense_store(const GemmArgs& p, int m, int n, float v0, float v1) {
     else p.out_f32[o] = rr;
     return;
   }
+  if (p.gate) {
+    const float gs = 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
+    v0 *= gs; v1 *= gs;
+  }
   if (p.rowbias) {
     const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.rowbias + (int64_t)(m % p.rowbias_mod) * p.N + n));
     v0 += b.x; v1 += b.y;
@@ -270,6 +274,7 @@ __global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_
           continue;
         }
         if (n < p.N && b < p.M) {
+          if (p.gate) v *= 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
           if (p.resid) v += p.resid[(int64_t)b * p.ldr + n];
           const int64_t o = (int64_t)b * p.ldo + n;
           if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(v);

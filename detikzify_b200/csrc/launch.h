@@ -31,6 +31,8 @@ struct GemmArgs {
   float* out_f32;             // exactly one of out_f32 / out_bf16 is non-null
   bf16* out_bf16;
   int64_t ldo;
+  // gated residual (TikZero cross layers): v = sigmoid(*gate) * act(acc + bias) before the residual add; null = off
+  const bf16* gate;
 };
 cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter);   // dispatches wgmma / mma.sync
 cudaError_t launch_gemm_mma(const GemmArgs& a, cudaStream_t s, uint64_t* counter);
@@ -73,6 +75,11 @@ cudaError_t launch_flash_attn(const AttnArgs& a, cudaStream_t s, uint64_t* count
 bool attn_tc_supported();
 int attn_tc_vt_cols(int N);
 cudaError_t launch_attn_tc(const bf16* qkv, bf16* vT, bf16* o, int B, int heads, int N, float scale, cudaStream_t s, uint64_t* counter);
+// cross-attention of the TikZero adapter on the same wgmma kernel: q bf16 [B*N, heads*72]; kv bf16 [B*Tk, 2*heads*72] (k | v
+// column blocks), image b attends to its first klen[b] (1..Tk) caption rows; vT scratch bf16 [B*heads*80, attn_tc_vt_cols(Tk)]
+constexpr int XATTN_MAX_B = 64;
+cudaError_t launch_xattn_tc(const bf16* q, const bf16* kv, const int* klen_host, int Tk, bf16* vT, bf16* o, int B, int heads,
+                            int N, float scale, cudaStream_t s, uint64_t* counter);
 
 // ---------------------------------------------------------------- row-wise / elementwise
 // y = LN(x) * w + b  (fp32 stats); x fp32 [M, D]; writes bf16 and/or fp32 outputs
@@ -96,6 +103,14 @@ cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, con
 cudaError_t launch_rope_kv_prefill(const float* qkv, int T, int start_pos, int heads, int kv_heads,
                                    const float* rope_cs, bf16* q_out, bf16* kcache, bf16* vcache,
                                    int max_len, cudaStream_t s, uint64_t* counter);
+// head_dim 64 prefill without a KV slot (caption encoder): qkv fp32 [T, (heads+2kv_heads)*64] -> roped q bf16 [T, heads*64],
+// roped k bf16 [T, kv_heads*64], v bf16 [T, kv_heads*64]; rope_cs fp32 [T, 32, 2]
+cudaError_t launch_rope_qkv64(const float* qkv, int T, int heads, int kv_heads, const float* rope_cs, bf16* q, bf16* k, bf16* v,
+                              cudaStream_t s, uint64_t* counter);
+// per-head LayerNorm (affine over head_dim, fp32 stats): in bf16 [M, heads*hd] row stride ld_in -> out (may alias in), ld_out
+cudaError_t launch_head_layernorm(const bf16* in, int64_t ld_in, const bf16* w, const bf16* b, float eps, int M, int heads,
+                                  int hd, bf16* out, int64_t ld_out, cudaStream_t s, uint64_t* counter);
+cudaError_t launch_cast_bf16_f32(const bf16* in, float* out, int64_t n, cudaStream_t s, uint64_t* counter);
 
 // ---------------------------------------------------------------- decode (batch of single tokens)
 enum { GEMV_STORE = 0, GEMV_ADD = 1, GEMV_GLU = 2, GEMV_QKV = 3 };

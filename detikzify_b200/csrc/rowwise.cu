@@ -217,6 +217,75 @@ __global__ void __launch_bounds__(64) rope_kv_prefill_kernel(const float* __rest
   }
 }
 
+// ---- head_dim 64 RoPE of the caption encoder (rotate-half, HF modeling_llama.py), no cache: grid (T, heads + 2*kv_heads),
+//      32 threads: thread i handles the pair (i, i+32).
+__global__ void __launch_bounds__(32) rope_qkv64_kernel(const float* __restrict__ qkv, int heads, int kv_heads,
+                                                        const float* __restrict__ rope_cs, bf16* __restrict__ q,
+                                                        bf16* __restrict__ k, bf16* __restrict__ v) {
+  const int t = blockIdx.x, hh = blockIdx.y, i = threadIdx.x;
+  const int row = (heads + 2 * kv_heads) * 64;
+  const float* src = qkv + (int64_t)t * row + hh * 64;
+  const float a = src[i], b = src[i + 32];
+  const float2 cs = *reinterpret_cast<const float2*>(rope_cs + ((int64_t)t * 32 + i) * 2);
+  bf16* d;
+  if (hh < heads) d = q + (int64_t)t * heads * 64 + hh * 64;
+  else if (hh < heads + kv_heads) d = k + (int64_t)t * kv_heads * 64 + (hh - heads) * 64;
+  else {
+    d = v + (int64_t)t * kv_heads * 64 + (hh - heads - kv_heads) * 64;
+    d[i] = __float2bfloat16_rn(a);
+    d[i + 32] = __float2bfloat16_rn(b);
+    return;
+  }
+  d[i] = __float2bfloat16_rn(a * cs.x - b * cs.y);
+  d[i + 32] = __float2bfloat16_rn(b * cs.x + a * cs.y);
+}
+
+// ---- per-head LayerNorm (q_norm / k_norm of the TikZero cross-attention: nn.LayerNorm(head_dim) after the head split).
+//      One warp per (row, head); hd even and <= 128: lane j holds the pairs j and j + 32; fp32 two-pass statistics.
+__global__ void __launch_bounds__(256) head_layernorm_kernel(const bf16* in, int64_t ld_in, const bf16* __restrict__ w,
+                                                             const bf16* __restrict__ b, float eps, int M, int heads, int hd,
+                                                             bf16* out, int64_t ld_out) {
+  const int64_t item = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (item >= (int64_t)M * heads) return;
+  const int64_t row = item / heads;
+  const int h = (int)(item % heads);
+  const bf16* src = in + row * ld_in + h * hd;
+  float2 x[2];
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = 2 * (lane + 32 * j);
+    x[j] = i < hd ? unpack_bf16x2(*reinterpret_cast<const uint32_t*>(src + i)) : make_float2(0.f, 0.f);
+    s += x[j].x + x[j].y;
+  }
+  const float mean = warp_sum(s) / hd;
+  float q = 0.f;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    if (2 * (lane + 32 * j) < hd) {
+      const float a = x[j].x - mean, c = x[j].y - mean;
+      q += a * a + c * c;
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(q) / hd + eps);
+  bf16* dst = out + row * ld_out + h * hd;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int i = 2 * (lane + 32 * j);
+    if (i >= hd) continue;
+    const float2 ww = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(w + i));
+    const float2 bb = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(b + i));
+    *reinterpret_cast<uint32_t*>(dst + i) =
+        pack_bf16x2((x[j].x - mean) * rstd * ww.x + bb.x, (x[j].y - mean) * rstd * ww.y + bb.y);
+  }
+}
+
+__global__ void __launch_bounds__(256) cast_bf16_f32_kernel(const bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (i < n) out[i] = __bfloat162float(in[i]);
+}
+
 // ---- batched-decode RoPE + KV-cache append: row b belongs to sequence slots[b] at position pos[b]
 //      (HF modeling_llama.py:124-168; DynamicCache.update). grid (B, heads + 2*kv_heads); 64 threads.
 __global__ void __launch_bounds__(64) rope_kv_decode_kernel(const float* __restrict__ qkv, const int* __restrict__ slots,
@@ -344,6 +413,25 @@ cudaError_t launch_rope_kv_prefill(const float* qkv, int T, int start_pos, int h
   dim3 grid(T, heads + 2 * kv_heads);
   rope_kv_prefill_kernel<<<grid, 64, 0, s>>>(qkv, T, start_pos, heads, kv_heads, rope_cs, q_out, kcache, vcache,
                                              max_len);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
+cudaError_t launch_rope_qkv64(const float* qkv, int T, int heads, int kv_heads, const float* rope_cs, bf16* q, bf16* k, bf16* v,
+                              cudaStream_t s, uint64_t* counter) {
+  rope_qkv64_kernel<<<dim3(T, heads + 2 * kv_heads), 32, 0, s>>>(qkv, heads, kv_heads, rope_cs, q, k, v);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
+cudaError_t launch_head_layernorm(const bf16* in, int64_t ld_in, const bf16* w, const bf16* b, float eps, int M, int heads,
+                                  int hd, bf16* out, int64_t ld_out, cudaStream_t s, uint64_t* counter) {
+  if ((hd & 1) || hd > 128 || (ld_in & 1) || (ld_out & 1)) return cudaErrorInvalidValue;
+  const int64_t items = (int64_t)M * heads;
+  head_layernorm_kernel<<<(unsigned)((items + 7) / 8), 256, 0, s>>>(in, ld_in, w, b, eps, M, heads, hd, out, ld_out);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
+cudaError_t launch_cast_bf16_f32(const bf16* in, float* out, int64_t n, cudaStream_t s, uint64_t* counter) {
+  cast_bf16_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(in, out, n);
   if (counter) ++*counter;
   return cudaGetLastError();
 }

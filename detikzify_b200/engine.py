@@ -280,6 +280,59 @@ class Engine:
         tokens, _ = self.vit_encode(pixels, want_pooled=False)
         return self.project(tokens)
 
+    # ------------------------------------------------------------------ TikZero adapter
+    def adapter_attach(self, cacfg, arena: torch.Tensor):
+        """Attach the adapter arena (bf16, ``adapter_weight_table`` layout); the engine borrows it until detach."""
+        self.adapter_arena = arena.to(self.device).contiguous()
+        self.cacfg = cacfg
+        self._check(self.lib.dtk_adapter_attach(self._h, C.byref(cacfg), self._ptr(self.adapter_arena),
+                                                C.c_uint64(self.adapter_arena.numel() * self.adapter_arena.element_size())),
+                    "dtk_adapter_attach")
+
+    def adapter_detach(self):
+        self._check(self.lib.dtk_adapter_detach(self._h), "dtk_adapter_detach")
+        self.adapter_arena = self.cacfg = None
+
+    def text_encode(self, ids: torch.Tensor, want_hidden: bool = False):
+        """One unpadded caption, ids int64 [T] -> (hidden fp32 [T,E] | None, caption states fp32 [T,D])."""
+        ids = torch.as_tensor(ids).to(self.device, torch.int64).contiguous().view(-1)
+        T = ids.numel()
+        hidden = torch.empty(T, self.cacfg.hidden, device=self.device, dtype=torch.float32) if want_hidden else None
+        cond = torch.empty(T, self.D, device=self.device, dtype=torch.float32)
+        self._check(self.lib.dtk_text_encode(self._h, self._ptr(ids), T, self._ptr(hidden), self._ptr(cond), self._stream()),
+                    "dtk_text_encode")
+        return hidden, cond
+
+    def vit_encode_cond(self, pixels: torch.Tensor, captions: Sequence[torch.Tensor], want_tokens: bool = True,
+                        want_pooled: bool = True):
+        """ViT with the adapter's cross layers: image b conditioned on caption ids ``captions[b]`` (unpadded int64 [T_b])."""
+        pixels = pixels.to(self.device, torch.float32).contiguous()
+        B = pixels.shape[0]
+        assert len(captions) == B, (len(captions), B)
+        lens = [int(c.numel()) for c in captions]
+        Tmax = max(lens)
+        cond = torch.zeros(B, Tmax, self.D, device=self.device, dtype=torch.float32)
+        for b, ids in enumerate(captions):
+            cond[b, : lens[b]] = self.text_encode(ids)[1]
+        return self.vit_encode_states(pixels, cond, lens, want_tokens, want_pooled)
+
+    def vit_encode_states(self, pixels: torch.Tensor, cond: torch.Tensor, lens: Sequence[int], want_tokens: bool = True,
+                          want_pooled: bool = True):
+        """pixels fp32 [B,3,S,S], caption states fp32 [B,Tmax,D] (``text_encode`` output, caption b valid in rows < lens[b])."""
+        pixels = pixels.to(self.device, torch.float32).contiguous()
+        cond = cond.to(self.device, torch.float32).contiguous()
+        B, Tmax = pixels.shape[0], cond.shape[1]
+        tokens = torch.empty(B, self.N, self.D, device=self.device, dtype=torch.float32) if want_tokens else None
+        pooled = torch.empty(B, self.D, device=self.device, dtype=torch.float32) if want_pooled else None
+        cl = (C.c_int * B)(*lens)
+        self._check(self.lib.dtk_vit_encode_cond(self._h, self._ptr(pixels), B, self._ptr(cond), cl, Tmax, self._ptr(tokens),
+                                                 self._ptr(pooled), self._stream()), "dtk_vit_encode_cond")
+        return tokens, pooled
+
+    def image_embeds_cond(self, pixels: torch.Tensor, captions: Sequence[torch.Tensor]) -> torch.Tensor:
+        tokens, _ = self.vit_encode_cond(pixels, captions, want_pooled=False)
+        return self.project(tokens)
+
     # ------------------------------------------------------------------ KV slots
     def seq_alloc(self) -> int:
         s = C.c_int(-1)

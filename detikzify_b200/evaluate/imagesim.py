@@ -10,6 +10,10 @@ EMD = min-cost perfect matching / N, solved exactly by ``scipy.optimize.linear_s
 suite checks it against the transport LP. The cost matrix (fp64 pairwise cosines) is built on the device, the N x N
 assignment runs on the host like the reference's simplex (about 23 ms per pair at the v2 size N = 900).
 
+TikZero (reference imagesim.py:61-85,87-142): with a text-conditioning adapter loaded, a side that carries a caption (the target
+``img2`` or no image, plus ``text2``) is encoded by the adapted tower; the rendered candidates stay on the plain tower. The
+conditioned target is encoded once per (figure, caption) and reused for every candidate.
+
 torchmetrics is not a dependency here: the ``update / compute / reset`` protocol the MCTS driver uses
 (infer/generate.py:293-298) is implemented directly.
 """
@@ -27,11 +31,13 @@ from ..util.image import expand, load
 class ImageSim:
     higher_is_better = True
 
-    def __init__(self, model=None, processor=None, mode: str = "cos", preprocess: bool = True, **_):
+    def __init__(self, model=None, processor=None, mode: str = "cos", preprocess: bool = True, tokenizer=None, **_):
         if mode not in ("cos", "cos_avg", "emd"):
             raise NotImplementedError(f"ImageSim mode {mode!r} is not supported (cos / cos_avg / emd)")
         self.model, self.processor = model, processor
+        self.tokenizer = tokenizer          # caption tokenizer of a TikZero adapter (None: captions are refused)
         self.mode, self.preprocess = mode, preprocess
+        self._cond = None                   # ((image key, caption), features) of the last conditioned side
         self.reset()
 
     def __str__(self):
@@ -42,20 +48,40 @@ class ImageSim:
         from ..util.generation import unwrap_processor
         kwargs.pop("sync_on_compute", None)
         mode = getattr(model.config, "pooling_mode", "emd") if mode is None else mode
-        return cls(model=model.model.vision_model, processor=unwrap_processor(processor).image_processor, mode=mode, **kwargs)
+        tokenizer = processor.tokenizer if hasattr(model, "adapter") and hasattr(processor, "processor") else None
+        return cls(model=model.model.vision_model, processor=unwrap_processor(processor).image_processor, mode=mode,
+                   tokenizer=tokenizer, **kwargs)
 
-    def get_vision_features(self, image: Union[Image.Image, str]) -> torch.Tensor:
-        image = load(image)
-        if self.preprocess:
-            image = expand(image, max(image.size), do_trim=True)
+    def _features(self, out) -> torch.Tensor:
+        if self.mode == "cos":
+            return out.pooler_output.squeeze()
+        if self.mode == "cos_avg":
+            return out.last_hidden_state.squeeze().mean(dim=0)
+        return out.last_hidden_state.squeeze()
+
+    def get_vision_features(self, image: Optional[Union[Image.Image, str]] = None, text: Optional[str] = None) -> torch.Tensor:
+        if image is None and text is None:
+            raise ValueError("either an image or a text is needed")
+        if image is not None:
+            image = load(image)
+            if self.preprocess:
+                image = expand(image, max(image.size), do_trim=True)
+        if text is None:
+            with torch.inference_mode():
+                pixel_values = self.processor(images=image, return_tensors="pt")["pixel_values"]
+                return self._features(self.model(pixel_values=pixel_values))
+        if self.tokenizer is None:
+            raise ValueError("a caption needs an ImageSim built (from_detikzify) from a model with a loaded TikZero adapter")
+        key = (None if image is None else (image.size, hash(image.tobytes())), text)
+        if self._cond is not None and self._cond[0] == key:
+            return self._cond[1]
         with torch.inference_mode():
-            pixel_values = self.processor(images=image, return_tensors="pt")["pixel_values"]
-            out = self.model(pixel_values=pixel_values)
-            if self.mode == "cos":
-                return out.pooler_output.squeeze()
-            if self.mode == "cos_avg":
-                return out.last_hidden_state.squeeze().mean(dim=0)
-            return out.last_hidden_state.squeeze()
+            enc = self.tokenizer(text=[text], truncation=True, return_tensors="pt")
+            pixel_values = self.processor(images=image, return_tensors="pt")["pixel_values"] if image is not None else None
+            feats = self._features(self.model(pixel_values=pixel_values, adapter_input_ids=enc["input_ids"],
+                                              adapter_attention_mask=enc["attention_mask"]))
+        self._cond = (key, feats)
+        return feats
 
     @staticmethod
     def _emd_similarity(f1: torch.Tensor, f2: torch.Tensor) -> float:
@@ -70,18 +96,24 @@ class ImageSim:
         rows, cols = linear_sum_assignment(dists)
         return 2 * tanh(-float(dists[rows, cols].sum()) / dists.shape[0]) + 1
 
-    def get_similarity(self, img1=None, img2=None, **_) -> float:
-        f1, f2 = self.get_vision_features(img1), self.get_vision_features(img2)
+    def get_similarity(self, img1=None, img2=None, text1=None, text2=None, **_) -> float:
+        f1, f2 = self.get_vision_features(img1, text1), self.get_vision_features(img2, text2)
         if f1.ndim > 1:
             return self._emd_similarity(f1, f2)
         return F.cosine_similarity(f1.double(), f2.double(), dim=0).item()
 
-    def get_similarities(self, candidates: List[Union[Image.Image, str]], reference: Union[Image.Image, str]) -> List[float]:
+    def get_similarities(self, candidates: List[Union[Image.Image, str]], reference: Optional[Union[Image.Image, str]],
+                         text: Optional[str] = None) -> List[float]:
         """SelfSim of several candidate renders against one reference figure: all images go through ONE batched ViT pass
         (the renders of a batch of parallel MCTS rollouts), the fp64 cosines are taken on the device and read back with a
-        single transfer. Same values as ``get_similarity`` per pair (reference evaluate/imagesim.py:91-125)."""
+        single transfer. Same values as ``get_similarity`` per pair (reference evaluate/imagesim.py:91-125). With ``text``
+        (TikZero) the reference side (``reference`` or no image, plus the caption) is encoded by the adapted tower, once per
+        (figure, caption), and the batch holds the candidates only."""
+        target = None
+        if text is not None:
+            target = self.get_vision_features(reference, text)
         images = []
-        for image in [reference, *candidates]:
+        for image in ([] if target is not None else [reference]) + list(candidates):
             image = load(image)
             if self.preprocess:
                 image = expand(image, max(image.size), do_trim=True)
@@ -98,17 +130,27 @@ class ImageSim:
             out = self.model(pixel_values=pixel_values)
             if self.mode == "emd":
                 tokens = out.last_hidden_state
+                if target is not None:
+                    return [self._emd_similarity(tokens[i], target) for i in range(tokens.shape[0])]
                 return [self._emd_similarity(tokens[i], tokens[0]) for i in range(1, tokens.shape[0])]
             feats = out.pooler_output if self.mode == "cos" else out.last_hidden_state.mean(dim=1)
             feats = feats.double()
+            if target is not None:
+                return F.cosine_similarity(feats, target.double()[None].expand_as(feats), dim=1).tolist()
             return F.cosine_similarity(feats[1:], feats[:1].expand_as(feats[1:]), dim=1).tolist()
 
     def update(self, img1=None, img2=None, text1=None, text2=None):
-        imgs1 = img1 if isinstance(img1, list) else [img1]
-        imgs2 = img2 if isinstance(img2, list) else [img2]
-        assert len(imgs1) == len(imgs2) and all(i is not None for i in imgs1 + imgs2)
-        for a, b in zip(imgs1, imgs2):
-            self.score += self.get_similarity(a, b)
+        """reference imagesim.py:127-142: each side needs an image or a text; lists pair up element-wise."""
+        inputs = {}
+        for key, value in dict(img1=img1, img2=img2, text1=text1, text2=text2).items():
+            if value is not None:
+                inputs[key] = value if isinstance(value, list) else [value]
+        if {"img1", "text1"}.isdisjoint(inputs) or {"img2", "text2"}.isdisjoint(inputs):
+            raise ValueError("each side of the comparison needs an image or a text")
+        if len(set(map(len, inputs.values()))) != 1:
+            raise ValueError("img1 / img2 / text1 / text2 lists must have the same length")
+        for values in zip(*inputs.values()):
+            self.score += self.get_similarity(**dict(zip(inputs.keys(), values)))
             self.n_samples += 1
 
     def compute(self) -> float:

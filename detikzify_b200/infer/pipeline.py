@@ -41,7 +41,8 @@ Numeric = Union[int, float]
 
 
 def has_adapter(model) -> bool:
-    """reference detikzify/model/adapter/__init__.py:6-7 (text-conditioning adapter; not supported here)."""
+    """reference detikzify/model/adapter/__init__.py:6-7: True once ``detikzify_b200.model.adapter.load`` attached the TikZero
+    text-conditioning adapter to the model."""
     return hasattr(model, "adapter")
 
 
@@ -215,6 +216,8 @@ class DetikzifyGenerator:
         self.control = control or ExplicitAbort()
         enc = processor(images=self.image, text=self.text, text_kwargs={"truncation": True}, return_tensors="pt")
         self.pixel_values = enc.get("pixel_values")       # preprocessed once per figure (the reference re-runs it per rollout)
+        # caption of a TikZero adapter (reference infer/generate.py:209-227 forwards the adapter_* keys to every generate call)
+        self.adapter_kwargs = {k: enc[k] for k in ("adapter_input_ids", "adapter_attention_mask") if k in enc}
         root_ids = enc.input_ids.to(model.device).squeeze()
         self.montecarlo = MonteCarlo(root_node=WideNode(root_ids, exploration=self.exploration))
         self.montecarlo.child_finder = self.child_finder
@@ -257,6 +260,7 @@ class DetikzifyGenerator:
                 begin_suppress_tokens=[self.model.config.text_config.eos_token_id],
                 pixel_values=self.pixel_values,
                 streamer=streamers,
+                **self.adapter_kwargs,
                 **self.gen_kwargs,
                 **gen_kwargs,
             ).squeeze()
@@ -324,13 +328,15 @@ class DetikzifyGenerator:
                             input_ids=starts[i].token_ids.unsqueeze(0), pixel_values=self.pixel_values,
                             bad_words_ids=[[self.model.config.image_token_id]],
                             begin_suppress_tokens=[self.model.config.text_config.eos_token_id],
-                            streamer=st, stopping_criteria=StoppingCriteriaList([trackers[i]]), **self.gen_kwargs)
+                            streamer=st, stopping_criteria=StoppingCriteriaList([trackers[i]]), **self.adapter_kwargs,
+                            **self.gen_kwargs)
                 else:
                     self.model.generate_batch(
                         [starts[i].token_ids for i in live], pixel_values=self.pixel_values,
                         bad_words_ids=[[self.model.config.image_token_id]],
                         begin_suppress_tokens=[self.model.config.text_config.eos_token_id],
-                        streamers=streamers, stopping_criteria=[[trackers[i]] for i in live], **self.gen_kwargs)
+                        streamers=streamers, stopping_criteria=[[trackers[i]] for i in live], **self.adapter_kwargs,
+                        **self.gen_kwargs)
         elif self.streamer is not None:
             self.streamer.end()
         if self.control.should_stop:
@@ -366,7 +372,8 @@ class DetikzifyGenerator:
         rewards: List[Numeric] = [-1] * len(docs)
         idx = [i for i, ok in enumerate(scorable) if ok]
         if len(idx) > 1 and hasattr(self.metric, "get_similarities"):
-            values = self.metric.get_similarities([docs[i].rasterize() for i in idx], self.image)
+            values = self.metric.get_similarities([docs[i].rasterize() for i in idx], self.image,
+                                                  **({"text": self.text} if self.text is not None else {}))
             for i, v in zip(idx, values):
                 rewards[i] = v
         else:
@@ -452,6 +459,9 @@ class DetikzifyPipeline:
     def simulate(self, image=None, text: Optional[str] = None, preprocess: bool = True,
                  expansions: Optional[Numeric] = None, timeout: Optional[int] = None, **gen_kwargs):
         self.check_inputs(image, text)
+        if text is not None and isinstance(self.metric, ImageSim) and self.metric.tokenizer is None:
+            raise ValueError("SelfSim with a caption encodes the caption side with the adapted tower: create the pipeline "
+                             "after adapter.load(model, processor)")
         generator = DetikzifyGenerator(
             model=self.model, processor=self.processor, metric=self.metric, mcts_timeout=timeout or None,
             image=self.load(image, preprocess=preprocess) if image is not None else None, text=text,

@@ -50,13 +50,25 @@ class DetikzifyVisionModel:
         self._owner = owner
         self.config = owner.config.vision_config
 
-    def __call__(self, pixel_values: torch.Tensor, **_) -> VisionOutput:
-        return self.forward(pixel_values)
+    def __call__(self, pixel_values: Optional[torch.Tensor] = None, adapter_input_ids=None, adapter_attention_mask=None,
+                 **_) -> VisionOutput:
+        return self.forward(pixel_values, adapter_input_ids, adapter_attention_mask)
 
-    def forward(self, pixel_values: torch.Tensor) -> VisionOutput:
+    def forward(self, pixel_values: Optional[torch.Tensor] = None, adapter_input_ids=None,
+                adapter_attention_mask=None) -> VisionOutput:
+        """With ``adapter_input_ids`` (TikZero) the tower runs with the adapter's cross layers, on the clamped dummy input
+        when there is no image (reference modeling_adapter.py:473-491, used by SelfSim for the caption side)."""
         o = self._owner
+        caps = None
+        if adapter_input_ids is not None:
+            caps = o._captions(adapter_input_ids, adapter_attention_mask)
+            if pixel_values is None:
+                pixel_values = o.adapter.dummy_pixels().expand(len(caps), -1, -1, -1)
         with o._lock, o._on_stream():
-            tokens, pooled = o.engine.vit_encode(pixel_values)
+            if caps is None:
+                tokens, pooled = o.engine.vit_encode(pixel_values)
+            else:
+                tokens, pooled = o.engine.vit_encode_cond(pixel_values, [torch.tensor(c) for c in caps])
             # cast on the engine stream, before the sync: a tensor must not leave the side stream while work on it is pending
             tokens, pooled = tokens.to(o.dtype), pooled.to(o.dtype)
             o._sync()
@@ -110,7 +122,7 @@ class DetikzifyForCausalLM:
         self._kv: List[_KVSlot] = [_KVSlot(self.engine.seq_alloc())]
         self._kv_cur = self._kv[0]
         self._tick = 0
-        self._img_cache = None                  # (pixel tensor on device, image embeds [P,H])
+        self._img_cache = None                  # (pixel tensor on device, image embeds [P,H], caption ids or None)
         self._call_counter = 0
 
     # (kept for callers that reset the cache: ``model._slot_tokens = []`` forgets every cached prefix)
@@ -187,20 +199,50 @@ class DetikzifyForCausalLM:
     def get_model(self):
         return self.model
 
-    # ---- image features (cached per pixel tensor) ----------------------------------------------
-    def _image_embeds(self, pixel_values: torch.Tensor) -> torch.Tensor:
+    # ---- image features (cached per pixel tensor and caption) -----------------------------------
+    def _image_embeds(self, pixel_values: torch.Tensor, caption: Optional[List[int]] = None) -> torch.Tensor:
         pix = pixel_values.to(self.device, torch.float32, non_blocking=True)
         if pix.dim() == 3:
             pix = pix[None]
         if pix.shape[0] != 1:
             raise ValueError("generate() supports a single image (batch size 1), like the reference's streamers")
+        key = tuple(caption) if caption is not None else None
         cached = self._img_cache
-        if cached is not None and cached[0].shape == pix.shape and torch.equal(cached[0], pix):
+        if cached is not None and cached[2] == key and cached[0].shape == pix.shape and torch.equal(cached[0], pix):
             return cached[1]
-        emb = self.engine.image_embeds(pix)[0]
-        self._img_cache = (pix.clone(), emb)
-        self._slot_tokens = []  # KV of the image prefix is stale for a new image
+        emb = (self.engine.image_embeds(pix) if key is None else self.engine.image_embeds_cond(pix, [torch.tensor(key)]))[0]
+        self._img_cache = (pix.clone(), emb, key)
+        self._slot_tokens = []  # KV of the image prefix is stale for a new image or caption
         return emb
+
+    # ---- TikZero adapter -------------------------------------------------------------------------
+    def has_adapter(self) -> bool:
+        return hasattr(self, "adapter")
+
+    def unload_cross_attn_adapter(self):
+        """Detach the adapter (reference modeling_adapter.py:528-532); image features conditioned on a caption are dropped."""
+        with self._lock:
+            self.engine.adapter_detach()
+            del self.adapter, self.embedding_model
+            self._img_cache = None
+            self._slot_tokens = []
+
+    def _captions(self, adapter_input_ids, adapter_attention_mask) -> List[List[int]]:
+        """Caption ids per row, padding removed (right padding: the valid rows of the causal embedder are the unpadded ones)."""
+        if not self.has_adapter():
+            raise ValueError("Got `adapter_input_ids` but no adapter is loaded!")
+        ids = torch.as_tensor(adapter_input_ids)
+        ids = ids[None] if ids.dim() == 1 else ids
+        mask = None if adapter_attention_mask is None else torch.as_tensor(adapter_attention_mask).reshape(ids.shape)
+        out = []
+        for r in range(ids.shape[0]):
+            row = ids[r] if mask is None else ids[r][mask[r].bool()]
+            if row.numel() == 0:
+                raise ValueError("empty caption")
+            if row.numel() > self.adapter.config.max_text:
+                raise ValueError(f"caption longer than {self.adapter.config.max_text} tokens (truncate it in the processor)")
+            out.append(row.tolist())
+        return out
 
     @staticmethod
     def _first(seq, default=-1) -> int:
@@ -219,8 +261,16 @@ class DetikzifyForCausalLM:
                  temperature: Optional[float] = None, top_p: Optional[float] = None, top_k: Optional[int] = None,
                  max_length: Optional[int] = None, max_new_tokens: Optional[int] = None,
                  do_sample: Optional[bool] = None, seed: Optional[int] = None, eos_token_id: Optional[int] = None,
-                 **ignored) -> torch.Tensor:
+                 adapter_input_ids=None, adapter_attention_mask=None, **ignored) -> torch.Tensor:
         cfg, eng = self.config, self.engine
+        caption = None
+        if adapter_input_ids is not None:
+            caps = self._captions(adapter_input_ids, adapter_attention_mask)
+            if len(caps) != 1:
+                raise ValueError("generate() is batch-1: pass one caption")
+            caption = caps[0]
+            if pixel_values is None:
+                pixel_values = self.adapter.dummy_pixels()
         gc = self.generation_config
         temperature = gc.temperature if temperature is None else temperature
         top_p = gc.top_p if top_p is None else top_p
@@ -249,7 +299,7 @@ class DetikzifyForCausalLM:
                 img_start = ids_host.index(patch)
                 if ids_host[img_start: img_start + n_patch_tokens] != [patch] * n_patch_tokens:
                     raise ValueError("The image patch tokens should be consecutive.")
-                img = self._image_embeds(pixel_values)
+                img = self._image_embeds(pixel_values, caption)
             elif pixel_values is None and n_patch_tokens:
                 # patch tokens without an image: their KV comes from plain embeddings. Forget the image identity too, so a
                 # later call WITH the same image re-validates nothing against these slots (ADVICE r1)
@@ -325,7 +375,7 @@ class DetikzifyForCausalLM:
                        max_new_tokens: Optional[int] = None, do_sample: Optional[bool] = None, seed: Optional[int] = None,
                        eos_token_id: Optional[int] = None, streamers: Optional[Sequence[Any]] = None,
                        stopping_criteria: Optional[Sequence[Any]] = None, share_prefix: bool = True,
-                       **ignored) -> List[torch.Tensor]:
+                       adapter_input_ids=None, adapter_attention_mask=None, **ignored) -> List[torch.Tensor]:
         """N independent sequences decoded in lock-step: parallel MCTS rollouts of one figure (``pixel_values`` [1,3,S,S]
         shared) or N figures (``pixel_values`` [N,3,S,S]). One batched decode step per token — the decoder weights are
         streamed once per step for all N sequences instead of once per sequence — with the same logits processors and
@@ -352,6 +402,13 @@ class DetikzifyForCausalLM:
         N = len(prompts)
         if N == 0:
             return []
+        captions = None
+        if adapter_input_ids is not None:
+            captions = self._captions(adapter_input_ids, adapter_attention_mask)
+            if len(captions) not in (1, N):
+                raise ValueError("adapter_input_ids must hold one caption (shared) or one caption per sequence")
+            if pixel_values is None:
+                pixel_values = self.adapter.dummy_pixels()
         if any(len(p) == 0 for p in prompts):
             raise ValueError("empty prompt")
         streamers = list(streamers) if streamers is not None else [None] * N
@@ -388,7 +445,13 @@ class DetikzifyForCausalLM:
                     pix = pix[None]
                 if pix.shape[0] not in (1, N):
                     raise ValueError("pixel_values must hold one image (shared) or one image per sequence")
-                imgs = eng.image_embeds(pix)
+                if captions is None:
+                    imgs = eng.image_embeds(pix)
+                else:   # one conditioned tower pass per distinct (image, caption) pairing
+                    if pix.shape[0] != len(captions):
+                        pix = pix.expand(N, *pix.shape[1:]).contiguous()
+                        captions = captions * N if len(captions) == 1 else captions
+                    imgs = eng.image_embeds_cond(pix, [torch.tensor(c) for c in captions])
             for i, st in enumerate(streamers):
                 if st is not None:
                     st.put(torch.tensor([prompts[i]], dtype=torch.int64))

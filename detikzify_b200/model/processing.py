@@ -254,6 +254,13 @@ class SyntheticTokenizer:
         if truncation:
             lim = max_length or self.model_max_length
             enc = [e[:lim] for e in enc]
+        if padding and padding != "do_not_pad":   # right padding to the longest sequence
+            n = max(len(e) for e in enc)
+            mask = [[1] * len(e) + [0] * (n - len(e)) for e in enc]
+            enc = [e + [self.pad_token_id] * (n - len(e)) for e in enc]
+            if return_tensors == "pt":
+                return BatchFeature(input_ids=torch.tensor(enc, dtype=torch.long), attention_mask=torch.tensor(mask, dtype=torch.long))
+            return BatchFeature(input_ids=enc, attention_mask=mask)
         if return_tensors == "pt":
             n = max(len(e) for e in enc)
             if any(len(e) != n for e in enc):
@@ -349,3 +356,52 @@ class DetikzifyProcessor:
     @property
     def model_input_names(self):
         return list(dict.fromkeys(self.tokenizer.model_input_names + self.image_processor.model_input_names))
+
+
+class AdapterProcessor:
+    """TikZero processor (reference model/adapter/processing_adapter.py:20-62): the caption goes through the embedder's
+    tokenizer with its keys prefixed ``adapter_``; without images the inner processor runs on ``DUMMY_IMAGE`` and only its
+    ``input_ids`` / ``attention_mask`` are kept (the model feeds the adapter's learned ``dummy_input`` to the tower instead)."""
+
+    attributes = ["processor", "tokenizer"]
+
+    def __init__(self, processor, tokenizer=None, **kwargs):
+        if processor is None:
+            raise ValueError("You need to specify a `processor`.")
+        if tokenizer is None:
+            raise ValueError("You need to specify a `tokenizer`.")
+        self.processor, self.tokenizer = processor, tokenizer
+
+    def __call__(self, text=None, images=None, **kwargs) -> BatchFeature:
+        from ..util import DUMMY_IMAGE
+        if images is None and text is None:
+            raise ValueError("Either `images` or `text` (or both) are expected as arguments to an `AdapterProcessor` instance.")
+        text_kwargs, images_kwargs = dict(kwargs.pop("text_kwargs", None) or {}), dict(kwargs.pop("images_kwargs", None) or {})
+        if text is None:
+            text_inputs = dict()
+        else:
+            text = [text] if isinstance(text, str) else list(text)
+            text_inputs = {f"adapter_{k}": v for k, v in self.tokenizer(text=text, **kwargs, **text_kwargs).items()}
+            if getattr(self.processor, "model_expects_text", False):
+                images_kwargs.update(text=text, add_bos_token=True)
+        if images is None:
+            image_inputs = self.processor(images=len(text) * [DUMMY_IMAGE], **kwargs, **images_kwargs)
+            image_inputs = {k: image_inputs[k] for k in ["input_ids", "attention_mask"] if k in image_inputs}
+        else:
+            if not isinstance(images, (list, tuple)):
+                images = [images]
+            image_inputs = self.processor(images=images, **kwargs, **images_kwargs)
+        if text is not None and images is not None and len(images) != len(text):
+            raise ValueError(f"Received {len(images)} images for {len(text)} prompts. "
+                             "Each prompt should be associated with an image.")
+        return BatchFeature({**image_inputs, **text_inputs})
+
+    def batch_decode(self, *args, **kwargs):
+        return self.processor.batch_decode(*args, **kwargs)
+
+    def decode(self, *args, **kwargs):
+        return self.processor.decode(*args, **kwargs)
+
+    @property
+    def model_input_names(self):
+        return list(dict.fromkeys(self.tokenizer.model_input_names + self.processor.model_input_names))

@@ -110,6 +110,37 @@ DTK_API const char* dtk_last_error(const dtk_engine* eng);
 DTK_API int dtk_vit_encode(dtk_engine* eng, const float* pixels, int B, float* tokens_out,
                    float* pooled_out, void* stream);
 
+/* ---- TikZero text conditioning (reference detikzify/model/adapter: a Llama-3.2-1B caption embedder, a connector E -> D and
+ *      one gated cross-attention layer before every cross_every_n-th ViT layer). The adapter weights live in a SECOND
+ *      contiguous bf16 arena whose layout the library defines (dtk_adapter_weight_*), attached to an existing engine. ---- */
+typedef struct dtk_adapter_config {
+  /* caption embedder (LlamaModel; head_dim must be 64) */
+  int32_t hidden, inter, layers, heads, kv_heads, head_dim, vocab;
+  float rms_eps, rope_theta, rope_factor;
+  int32_t rope_type;          /* as dtk_config.rope_type */
+  float rope_low_freq, rope_high_freq;
+  int32_t rope_orig_max_pos;
+  int32_t max_text;           /* longest caption (tokenizer model_max_length, 512) */
+  int32_t cross_every_n;      /* cross layer before vision layer l iff (l + 1) % cross_every_n == 0 */
+} dtk_adapter_config;
+
+/* weight table of the adapter arena; the vision dims (cross-layer widths, dummy image size) are the engine config's */
+DTK_API int dtk_adapter_weight_count(const dtk_config* cfg, const dtk_adapter_config* acfg);
+DTK_API int dtk_adapter_weight_get(const dtk_config* cfg, const dtk_adapter_config* acfg, int index, dtk_weight_info* out);
+DTK_API uint64_t dtk_adapter_arena_bytes(const dtk_config* cfg, const dtk_adapter_config* acfg);
+/* borrow `arena` (device) until dtk_adapter_detach / dtk_destroy; allocates the caption encoder's workspace */
+DTK_API int dtk_adapter_attach(dtk_engine* eng, const dtk_adapter_config* acfg, const void* arena, uint64_t arena_bytes);
+DTK_API int dtk_adapter_detach(dtk_engine* eng);
+/* caption encoder (reference adapter hook: embedding_model(...).last_hidden_state, then adapter.connect): ids device int64
+ * [T], 1 <= T <= max_text, one unpadded caption (with right padding and causal attention the valid rows of a padded batch
+ * are exactly this). hidden_out (may be NULL): fp32 [T, E] final-RMSNorm states (bf16-rounded, the connector's operand);
+ * cond_out: fp32 [T, D] connector output. */
+DTK_API int dtk_text_encode(dtk_engine* eng, const int64_t* ids, int T, float* hidden_out, float* cond_out, void* stream);
+/* ViT with the cross layers inserted: as dtk_vit_encode, conditioned on cond fp32 [B, Tmax, D] (dtk_text_encode output,
+ * caption b valid in rows [0, cond_len[b])); cond_len host int[B], 1 <= cond_len[b] <= Tmax <= max_text. */
+DTK_API int dtk_vit_encode_cond(dtk_engine* eng, const float* pixels, int B, const float* cond, const int* cond_len,
+                                int Tmax, float* tokens_out, float* pooled_out, void* stream);
+
 /* ---- image preprocessing on the device. Replaces DetikzifyImageProcessor.preprocess for images already uploaded as
  *      uint8 (detikzify/model/v1/processing_detikzify.py:242-251: bicubic resize to SxS, x 1/255, (x - mean) / std, CHW).
  *      rgb: device uint8 [h, w, 3]; the resize is Pillow's 8-bit resampler bit for bit: bounds_* int32 [S][2] = {first
@@ -218,6 +249,16 @@ DTK_API int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void
 /* ViT attention on wgmma: qkv bf16 [B*N, 3*heads*72] (q | k | v column blocks), vt_scratch bf16 [B*heads*80, ceil(N/128)*128],
  * o bf16 [B*N, heads*72]; non-causal, head_dim 72 */
 DTK_API int dtk_dbg_attn_tc(const void* qkv, void* vt_scratch, void* o, int B, int heads, int N, float scale, void* stream);
+/* TikZero cross-attention on wgmma: q bf16 [B*N, heads*72], kv bf16 [B*Tk, 2*heads*72] (k | v), image b attends to its
+ * first klen_host[b] keys (1..Tk, B <= 64); vt_scratch bf16 [B*heads*80, ceil(Tk/128)*128]; o bf16 [B*N, heads*72] */
+DTK_API int dtk_dbg_xattn_tc(const void* q, const void* kv, const int* klen_host, int Tk, void* vt_scratch, void* o, int B,
+                             int heads, int N, float scale, void* stream);
+/* per-head LayerNorm: x bf16 [M, heads*hd] -> out bf16 (same layout), affine w/b bf16 [hd] */
+DTK_API int dtk_dbg_head_layernorm(const void* x, const void* w, const void* b, float eps, int M, int heads, int hd, void* out,
+                                   void* stream);
+/* gated residual GEMM: out_f32 = resid + sigmoid(gate) * act(A W^T + bias); gate bf16 [1] device */
+DTK_API int dtk_dbg_gemm_gated(const void* A_bf16, const void* W_bf16, const void* bias_bf16, const void* gate_bf16,
+                               const float* resid, int M, int N, int K, int act, float* out_f32, void* stream);
 /* y = W[N,K] * rmsnorm?(x[K]) ; mode 0 store / 1 add / 2 glu (out[N/2]) */
 DTK_API int dtk_dbg_gemv(const void* W_bf16, const float* x, const void* norm_w_bf16, float eps,
                          int N, int K, int mode, float* out, void* stream);
