@@ -1,7 +1,8 @@
 // Flash attention (online softmax, fp32 statistics) on mma.sync tiles.
 //   * ViT self-attention: 16 heads x head_dim 72 (zero-padded to 80 in shared memory for the
 //     QK^T contraction), N = 729 keys, non-causal  — HF modeling_siglip.py:229-249,293-306.
-//   * LLaMA prefill: head_dim 128, causal over cached positions — HF modeling_llama.py:199-222.
+//   * LLaMA prefill: head_dim 128 or 64 (TinyLlama), causal over cached positions — HF modeling_llama.py:199-222;
+//     non-causal partials of the shared prefix of a batched decode step.
 //   * TikZero caption encoder (Llama-3.2-1B): head_dim 64, causal.
 // One CTA = 64 queries of one (batch, head); 4 warps x 16 query rows; K/V streamed in 64-key tiles
 // through a 2-stage cp.async ring. P is re-used straight from the score accumulators as the
@@ -212,7 +213,7 @@ __global__ void __launch_bounds__(ATHREADS) flash_attn_kernel(const AttnArgs p) 
       }
 #pragma unroll
       for (int i = 0; i < D / 8; ++i)
-        *reinterpret_cast<float2*>(p.part_o + pi * 128 + i * 8 + tq4 * 2) = make_float2(o[i][h * 2], o[i][h * 2 + 1]);
+        *reinterpret_cast<float2*>(p.part_o + pi * D + i * 8 + tq4 * 2) = make_float2(o[i][h * 2], o[i][h * 2 + 1]);
     }
     return;
   }
@@ -254,14 +255,15 @@ cudaError_t launch_t(const AttnArgs& a, cudaStream_t s) {
 cudaError_t launch_flash_attn(const AttnArgs& a, cudaStream_t s, uint64_t* counter) {
   if (a.Tq <= 0 || a.B <= 0) return cudaSuccess;
   if (a.part_o) {   // shared-prefix partials of a batched decode step
-    if (a.head_dim != 128 || a.causal || a.Tq > BQ || a.B != 1 || a.part_tiles <= 0 || a.Tk <= 0 || !a.part_ml) return cudaErrorInvalidValue;
+    if ((a.head_dim != 128 && a.head_dim != 64) || a.causal || a.Tq > BQ || a.B != 1 || a.part_tiles <= 0 || a.Tk <= 0 || !a.part_ml)
+      return cudaErrorInvalidValue;
     if (counter) ++*counter;
-    return launch_t<128, 128, false, true>(a, s);
+    return a.head_dim == 128 ? launch_t<128, 128, false, true>(a, s) : launch_t<64, 64, false, true>(a, s);
   }
   if (counter) ++*counter;
   if (a.head_dim == 72) return a.causal ? launch_t<72, 80, true, false>(a, s) : launch_t<72, 80, false, false>(a, s);
   if (a.head_dim == 128) return a.causal ? launch_t<128, 128, true, false>(a, s) : launch_t<128, 128, false, false>(a, s);
-  if (a.head_dim == 64 && a.causal) return launch_t<64, 64, true, false>(a, s);   // caption encoder (Llama-3.2-1B)
+  if (a.head_dim == 64 && a.causal) return launch_t<64, 64, true, false>(a, s);   // caption encoder, head_dim-64 decoders (prefill)
   return cudaErrorInvalidValue;
 }
 

@@ -17,7 +17,7 @@
 //     m16n8k16, fp32 accumulate) with the activation vector split into bf16 hi + lo parts (x = hi + lo to 2^-17)
 //     that occupy alternating columns of the B operand: one HMMA per k-step, fp32-grade GEMV; the ring slot is
 //     handed back as soon as its shared-memory reads are issued;
-//   * rows are grouped so that one thread's two accumulator rows (g, g+8) are a RoPE pair (i, i+64) or a
+//   * rows are grouped so that one thread's two accumulator rows (g, g+8) are a RoPE pair (i, i+HD/2) or a
 //     SwiGLU pair (gate_i, up_i): RMSNorm scale, RoPE + KV-cache write, SiLU*mul and residual add are all fused
 //     into the group epilogue; partial sums of a group's k-tiles are combined in a fixed order (deterministic);
 //     the epilogues of a phase run in PARALLEL behind a CTA barrier (warp w takes groups w, w + 8, ...), not on whichever
@@ -47,6 +47,7 @@ constexpr int MEGA_THREADS = (NCW + NPW) * 32;
 constexpr int CONSUMER_THREADS = NCW * 32;
 static_assert(NCW % NPW == 0, "slot ownership: NPW must divide NCW");
 constexpr int TILE_BYTES = 8192;             // ring slot = one weight tile = one 16-key K+V attention item
+constexpr int KV_V_OFF = 4096;               // byte offset of the V rows in an attention item (K rows at 0; 16 x HD x 2 B each)
 constexpr int NT = 104;                      // per-tile partial-sum entries (>= max tiles/group + tiles in flight)
 constexpr int NS = 72;                       // 256-column slices of a staged input vector (>= max tiles per group)
 constexpr int NG = 48;                       // per-group arrival counters / prefetched residual rows (>= groups in flight)
@@ -307,12 +308,21 @@ DTK_DEV float slices_rn(const float* slice_ss, int nslice, int K, float eps) {
 }
 
 // DBG = true: dev instrumentation (phase stamps, per-tile trace, timing-experiment flags) compiled in.
+// HD = decoder head_dim (64 or 128): the RoPE row pairing of the qkv epilogue, the KV item rows, the attention lanes per key
+// and the partial/merge scratch.
 // Both roles run ONE rolled loop over the 5 L + 1 phases of the token (qkv | attention | o | gate/up | down per layer,
 // then lm_head) with a single copy of the tile code and a run-time phase switch in the epilogue: the per-token
 // instruction footprint of a warp stays inside the SM's 32 KB instruction cache (the fully specialised version was
 // ~160 KB, re-fetched from L2 every layer: the first tiles of every phase ran 3-6x slower than the steady state).
-template <bool DBG>
+template <bool DBG, int HD>
 __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const MegaArgs p) {
+  constexpr int HALF = HD / 2;
+  constexpr int LPK = HD / 8;                // attention: lanes per key (8 bf16 each)
+  constexpr int NGRP = 32 / LPK;             // key groups per warp
+  constexpr int NST = NCW * NGRP;            // online-softmax states per CTA
+  constexpr int PS = HD + 4;                 // per-CTA partial record: o[HD], m, l (padded)
+  constexpr int PPL = HD / 64;               // (q, k, v) pairs per lane when warp 0 fetches a head's vectors
+  constexpr int HSH = HD == 128 ? 7 : 6;     // log2(HD): divisions of non-negative ints as shifts
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int c = blockIdx.x, G = gridDim.x;
@@ -322,11 +332,11 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
   uint4* xb = reinterpret_cast<uint4*>(actf);
   uint64_t* bars = reinterpret_cast<uint64_t*>(actf + p.act_floats);
   float* red = reinterpret_cast<float*>(bars + 2 * nslots);  // 16 floats
-  float* rope_s = red + 16;                                   // [64][2] cos/sin of this position
+  float* rope_s = red + 16;                                   // [HD/2][2] cos/sin of this position
   float* tpart = rope_s + 128;                                // [NT][16] per-tile partial sums
   int* gcnt = reinterpret_cast<int*>(tpart + NT * 16);        // [NG] (unused since the epilogues run behind a barrier; keeps the layout)
   float* rbuf = reinterpret_cast<float*>(gcnt + NG);          // [NG][16] residuals prefetched at a group's first tile
-  float* qkn = rbuf + NG * 16;                                // [3][128] q | new key | new value of the CTA's head
+  float* qkn = rbuf + NG * 16;                                // [3][HD] q | new key | new value of the CTA's head
   float* slice_ss = qkn + 384;                                // [NS] sum of squares of each staged slice (normed phases)
   uint32_t* slice_tag = reinterpret_cast<uint32_t*>(slice_ss + NS);   // [NS] phase tag of the data a slice holds
   const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + nslots);
@@ -343,9 +353,9 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
   const int pos = p.pos[0], slot = p.slots[0];
   int tok = p.tok[0];
   if (tok < 0 || tok >= p.V) tok = 0;
-  const int qd = p.heads * 128, kd = p.kv_heads * 128;
+  const int qd = p.heads * HD, kd = p.kv_heads * HD;
   if (tid < NS) slice_tag[tid] = (uint32_t)p.bar_base[1];   // the epoch: never a phase tag of this launch
-  if (tid < 128) rope_s[tid] = p.rope_cs[(int64_t)pos * 128 + tid];
+  if (tid < HD) rope_s[tid] = p.rope_cs[(int64_t)pos * HD + tid];
   __syncthreads();
   const AttnSplit as = attn_split(p, c, G, pos);
   const int kvh = as.head / (p.heads / p.kv_heads);
@@ -395,7 +405,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
         }
         // this phase's local tile list: weight tiles of the CTA's row groups, or (attention) the CTA's share of the
         // cached keys / values of the layer: item i = positions [j0 + 16 i, +16) of the CTA's kv head, K rows at slot
-        // offset 0 and V rows at 4096 (rows of one head are contiguous in the cache). Neither depends on this token, so
+        // offset 0 and V rows at KV_V_OFF (rows of one head are contiguous in the cache). Neither depends on this token, so
         // both stream ahead of the dependency chain and the phases read shared memory only.
         const bool attn = ph == PH_ATTN;
         const MegaMat& m = p.mat[mat_of(ph)];
@@ -403,7 +413,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
         if (!attn) phase_span(w, m, g0, cnt, nact);
         const int tpg = attn ? 1 : m.tpg;
         const int ntiles = attn ? as.n_items : cnt * tpg;
-        const int64_t kvo = (int64_t)l * p.kv_layer_stride + (int64_t)kvh * p.max_len * 128;
+        const int64_t kvo = (int64_t)l * p.kv_layer_stride + (int64_t)kvh * p.max_len * HD;
         const bf16* base = attn ? kv_slot + kvo
                                 : m.base + (int64_t)l * m.layer_stride + (int64_t)g0 * tpg * MEGA_TILE_ELEMS;
         // own tiles j = j0, j0 + NPW, ...
@@ -414,11 +424,11 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
             const uint32_t dst = ring_u32 + sl * TILE_BYTES, fb = full0 + 8 * sl;
             if (attn) {
               const int key0 = as.j0 + (int)j * 16;
-              const uint32_t bytes = (uint32_t)min(16, p.max_len - key0) * 256u;
-              const bf16* kb = (key0 < shlen ? kv_share + kvo : base) + (int64_t)key0 * 128;
+              const uint32_t bytes = (uint32_t)min(16, p.max_len - key0) * (uint32_t)(HD * 2);
+              const bf16* kb = (key0 < shlen ? kv_share + kvo : base) + (int64_t)key0 * HD;
               mbar_expect_tx(fb, 2 * bytes);
               bulk_g2s(dst, kb, bytes, fb);
-              bulk_g2s(dst + 4096, kb + p.kv_v_offset, bytes, fb);
+              bulk_g2s(dst + KV_V_OFF, kb + p.kv_v_offset, bytes, fb);
             } else {
               mbar_expect_tx(fb, TILE_BYTES);
               bulk_g2s(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb);
@@ -497,20 +507,30 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
       // keys/values arrive through the ring, and q / the new key and value are polled (by one warp) as tagged words of
       // this head only.
       if (as.active) {
-        const int hw = lane >> 4, l16 = lane & 15;
-        if (warp == 0) {   // one warp fetches q (and, in the head's last key range, the new key / value row): 64 pairs each
-          const float sl2 = 0.08838834764831845f * 1.4426950408889634f;  // 128^-1/2 * log2(e)
+        const int hw = lane >> (HSH - 3), l16 = lane & (LPK - 1);   // key group of the lane, lane inside the group
+        if (warp == 0) {   // one warp fetches q (and, in the head's last key range, the new key / value row): HD/2 pairs each
+          // head_dim^-1/2 * log2(e)
+          const float sl2 = (HD == 128 ? 0.08838834764831845f : 0.125f) * 1.4426950408889634f;
           float2* q2 = reinterpret_cast<float2*>(qkn);
-          const u64* qsrc = t_q + as.head * 128;
-          const u64* const ptr[6] = {qsrc + 2 * lane, qsrc + 2 * (lane + 32), t_kn + kvh * 128 + 2 * lane, t_kn + kvh * 128 + 2 * (lane + 32),
-                                     t_vn + kvh * 128 + 2 * lane, t_vn + kvh * 128 + 2 * (lane + 32)};
           const bool lastr = as.last != 0;
-          const bool on[6] = {true, true, lastr, lastr, lastr, lastr};
-          float2 v[6];
-          ld_pairs<6>(ptr, on, tag - 1, nowait, v);
-          q2[lane] = make_float2(v[0].x * sl2, v[0].y * sl2);
-          q2[lane + 32] = make_float2(v[1].x * sl2, v[1].y * sl2);
-          if (lastr) { q2[64 + lane] = v[2]; q2[96 + lane] = v[3]; q2[128 + lane] = v[4]; q2[160 + lane] = v[5]; }
+          const u64* ptr[3 * PPL];
+          bool on[3 * PPL];
+#pragma unroll
+          for (int u = 0; u < PPL; ++u) {
+            ptr[u] = t_q + as.head * HD + 2 * (lane + 32 * u);
+            ptr[PPL + u] = t_kn + kvh * HD + 2 * (lane + 32 * u);
+            ptr[2 * PPL + u] = t_vn + kvh * HD + 2 * (lane + 32 * u);
+            on[u] = true;
+            on[PPL + u] = lastr;
+            on[2 * PPL + u] = lastr;
+          }
+          float2 v[3 * PPL];
+          ld_pairs<3 * PPL>(ptr, on, tag - 1, nowait, v);
+#pragma unroll
+          for (int u = 0; u < PPL; ++u) {
+            q2[lane + 32 * u] = make_float2(v[u].x * sl2, v[u].y * sl2);
+            if (lastr) { q2[HALF + lane + 32 * u] = v[PPL + u]; q2[HD + lane + 32 * u] = v[2 * PPL + u]; }
+          }
         }
         consumer_sync();   // q is staged; every warp is past its last qkv tile (the merge scratch below aliases the staged vector)
         stamp(1);
@@ -522,7 +542,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
         float m = -INFINITY, lsum = 0.f, o[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) o[i] = 0.f;
-        // online softmax over FOUR keys at a time (per half-warp): the four dot products and their shuffle reductions are
+        // online softmax over FOUR keys at a time (per key group): the four dot products and their shuffle reductions are
         // independent chains, one rescale per batch instead of one per key
         auto keys4 = [&](const uint4 (&kr)[4], const uint4 (&vr)[4], const bool (&valid)[4]) {
           float s2[4];
@@ -536,7 +556,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
             s2[u] = d;
           }
 #pragma unroll
-          for (int st = 8; st > 0; st >>= 1)
+          for (int st = LPK / 2; st > 0; st >>= 1)
 #pragma unroll
             for (int u = 0; u < 4; ++u) s2[u] += __shfl_xor_sync(0xffffffffu, s2[u], st);
           float mx = m;
@@ -561,7 +581,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
           }
           m = mx;
         };
-        // ring items: 16 positions each; half-warp hw takes positions hw, hw + 2, ... of the item
+        // ring items: 16 positions each; key group hw takes positions hw, hw + NGRP, ... of the item (16 / NGRP / 4 batches of 4)
         {
           uint32_t j = ((uint32_t)warp + NCW - (w.nb & (NCW - 1))) & (NCW - 1);
           if ((int)j < as.n_items) {
@@ -577,18 +597,19 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
               cur_slot = sl;
               const uint32_t base = ring_u32 + sl * TILE_BYTES + l16 * 16;
               const int key0 = as.j0 + (int)j * 16;
-              uint4 kr[2][4], vr[2][4];
+              constexpr int KPG = 16 / NGRP;   // positions of the item per key group
+              uint4 kr[KPG / 4][4], vr[KPG / 4][4];
 #pragma unroll
-              for (int u = 0; u < 8; ++u) {
-                const uint32_t a = base + (uint32_t)(u * 2 + hw) * 256u;
+              for (int u = 0; u < KPG; ++u) {
+                const uint32_t a = base + (uint32_t)(u * NGRP + hw) * (uint32_t)(HD * 2);
                 asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(kr[u >> 2][u & 3].x), "=r"(kr[u >> 2][u & 3].y), "=r"(kr[u >> 2][u & 3].z), "=r"(kr[u >> 2][u & 3].w) : "r"(a));
-                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(vr[u >> 2][u & 3].x), "=r"(vr[u >> 2][u & 3].y), "=r"(vr[u >> 2][u & 3].z), "=r"(vr[u >> 2][u & 3].w) : "r"(a + 4096u));
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(vr[u >> 2][u & 3].x), "=r"(vr[u >> 2][u & 3].y), "=r"(vr[u >> 2][u & 3].z), "=r"(vr[u >> 2][u & 3].w) : "r"(a + (uint32_t)KV_V_OFF));
               }
               release();
 #pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const bool valid[4] = {key0 + (h * 4 + 0) * 2 + hw < as.j1, key0 + (h * 4 + 1) * 2 + hw < as.j1,
-                                       key0 + (h * 4 + 2) * 2 + hw < as.j1, key0 + (h * 4 + 3) * 2 + hw < as.j1};
+              for (int h = 0; h < KPG / 4; ++h) {
+                const bool valid[4] = {key0 + (h * 4 + 0) * NGRP + hw < as.j1, key0 + (h * 4 + 1) * NGRP + hw < as.j1,
+                                       key0 + (h * 4 + 2) * NGRP + hw < as.j1, key0 + (h * 4 + 3) * NGRP + hw < as.j1};
                 keys4(kr[h], vr[h], valid);
               }
               if (DBG && trow && lane == 0) trow[2] = clock64();
@@ -601,76 +622,77 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
         if (as.last && warp == 0 && hw == 0) {   // the key / value of the token being decoded (published by the qkv phase of this launch)
           float d = 0.f;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) d += q[i] * qkn[128 + l16 * 8 + i];
+          for (int i = 0; i < 8; ++i) d += q[i] * qkn[HD + l16 * 8 + i];
 #pragma unroll
-          for (int st = 8; st > 0; st >>= 1) d += __shfl_xor_sync(0x0000ffffu, d, st);
+          for (int st = LPK / 2; st > 0; st >>= 1) d += __shfl_xor_sync((1u << LPK) - 1u, d, st);
           const float mx = fmaxf(m, d), alpha = exp2f(m - mx), pj = exp2f(d - mx);
           lsum = lsum * alpha + pj;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) o[i] = o[i] * alpha + pj * qkn[256 + l16 * 8 + i];
+          for (int i = 0; i < 8; ++i) o[i] = o[i] * alpha + pj * qkn[2 * HD + l16 * 8 + i];
           m = mx;
         }
-        // merge the 16 half-warp states -> one partial per CTA
-        float* sm_m = actf;            // [16]
-        float* sm_l = actf + 16;       // [16]
-        float* sm_o = actf + 32;       // [16][128]
-        const int hidx = warp * 2 + hw;
+        // merge the NST key-group states -> one partial per CTA
+        float* sm_m = actf;              // [NST]
+        float* sm_l = actf + NST;        // [NST]
+        float* sm_o = actf + 2 * NST;    // [NST][HD]
+        const int hidx = warp * NGRP + hw;
         if (l16 == 0) { sm_m[hidx] = m; sm_l[hidx] = lsum; }
 #pragma unroll
-        for (int i = 0; i < 8; ++i) sm_o[hidx * 128 + l16 * 8 + i] = o[i];
+        for (int i = 0; i < 8; ++i) sm_o[hidx * HD + l16 * 8 + i] = o[i];
         consumer_sync();
         const bool owner = c < p.heads;   // the CTA of the head's first key range folds the head's partials
-        float* mg = actf + 32 + 16 * 128;   // [cph][132] (owner only)
-        if (tid < 128) {
+        float* mg = sm_o + NST * HD;      // [cph][PS] (owner only)
+        if (tid < HD) {
           float M = -INFINITY;
 #pragma unroll
-          for (int h = 0; h < 16; ++h) M = fmaxf(M, sm_m[h]);
+          for (int h = 0; h < NST; ++h) M = fmaxf(M, sm_m[h]);
           float Lt = 0.f, O = 0.f;
 #pragma unroll
-          for (int h = 0; h < 16; ++h) {
+          for (int h = 0; h < NST; ++h) {
             const float wgt = (sm_m[h] == -INFINITY) ? 0.f : exp2f(sm_m[h] - M);
             Lt += sm_l[h] * wgt;
-            O += sm_o[h * 128 + tid] * wgt;
+            O += sm_o[h * HD + tid] * wgt;
           }
           if (owner) {
             mg[tid] = O;
-            if (tid == 0) { mg[128] = M; mg[129] = Lt; }
+            if (tid == 0) { mg[HD] = M; mg[HD + 1] = Lt; }
           } else {
-            u64* pp = t_part + (int64_t)c * 132;
+            u64* pp = t_part + (int64_t)c * PS;
             st_tag(pp + tid, O, tag);
-            if (tid == 0) { st_tag(pp + 128, M, tag); st_tag(pp + 129, Lt, tag); }
+            if (tid == 0) { st_tag(pp + HD, M, tag); st_tag(pp + HD + 1, Lt, tag); }
           }
         }
         if (owner) {
           // fixed owner instead of "last CTA to arrive": no atomic round trip on the critical path; the partials are tagged,
           // the owner polls them (coalesced, with back-off) as soon as its own share is done
-          const int nw = (as.cph - 1) * 130;
+          constexpr int PW = HD + 2;   // words of a partial record
+          const int nw = (as.cph - 1) * PW;
           for (int i0 = 0; i0 < nw; i0 += 2 * CONSUMER_THREADS) {
             u64 wv2[2];
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
               const int i = i0 + u * CONSUMER_THREADS + tid;
-              if (i < nw) wv2[u] = ld_weak1(t_part + (int64_t)((i / 130 + 1) * p.heads + as.head) * 132 + (i % 130));
+              if (i < nw) wv2[u] = ld_weak1(t_part + (int64_t)((i / PW + 1) * p.heads + as.head) * PS + (i % PW));
             }
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
               const int i = i0 + u * CONSUMER_THREADS + tid;
-              if (i < nw) mg[(i / 130 + 1) * 132 + (i % 130)] = settle1(wv2[u], t_part + (int64_t)((i / 130 + 1) * p.heads + as.head) * 132 + (i % 130), tag, nowait);
+              if (i < nw) mg[(i / PW + 1) * PS + (i % PW)] = settle1(wv2[u], t_part + (int64_t)((i / PW + 1) * p.heads + as.head) * PS + (i % PW), tag, nowait);
             }
           }
           consumer_sync();
-          if (tid < 128) {
+          if (tid < HD) {
             float M = -INFINITY;
-            for (int r = 0; r < as.cph; ++r) M = fmaxf(M, mg[r * 132 + 128]);
+            for (int r = 0; r < as.cph; ++r) M = fmaxf(M, mg[r * PS + HD]);
             float Lt = 0.f, O = 0.f;
 #pragma unroll 1
             for (int r = 0; r < as.cph; ++r) {
-              const float mr = mg[r * 132 + 128];
+              const float mr = mg[r * PS + HD];
               const float wgt = (mr == -INFINITY) ? 0.f : exp2f(mr - M);
-              Lt += mg[r * 132 + 129] * wgt;
-              O += mg[r * 132 + tid] * wgt;
+              Lt += mg[r * PS + HD + 1] * wgt;
+              O += mg[r * PS + tid] * wgt;
             }
-            st_tag(t_att + as.head * 128 + tid, O / Lt, tag);
+            st_tag(t_att + as.head * HD + tid, O / Lt, tag);
           }
         }
       } else {
@@ -723,30 +745,31 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
               if (lane < 8) {
                 const int gi = g0 + (int)ek, r = lane;
                 if (ph == PH_QKV) {
-                  const int hb = gi >> 3, i = ((gi & 7) << 3) + r;      // 128-row block, index inside the half
-                  const int row0 = hb * 128 + i;
+                  constexpr int GPH = HALF / 8;                          // 16-row groups per head
+                  const int hb = gi >> (HSH - 4), i = ((gi & (GPH - 1)) << 3) + r;   // HD-row head block, index inside the half
+                  const int row0 = hb * HD + i;
                   const float a0 = v * rn, a1 = v1 * rn;
                   if (row0 < qd + kd) {
                     const float2 csn = *reinterpret_cast<const float2*>(rope_s + i * 2);
                     const float y0 = a0 * csn.x - a1 * csn.y, y1 = a1 * csn.x + a0 * csn.y;
-                    if (row0 < qd) { st_tag(t_q + row0, y0, tag); st_tag(t_q + row0 + 64, y1, tag); }
+                    if (row0 < qd) { st_tag(t_q + row0, y0, tag); st_tag(t_q + row0 + HALF, y1, tag); }
                     else {
-                      const int kh = (row0 - qd) >> 7;
-                      bf16* dd = p.kv + (int64_t)slot * p.kv_slot_stride + (int64_t)l * p.kv_layer_stride + ((int64_t)kh * p.max_len + pos) * 128;
+                      const int kh = (row0 - qd) >> HSH;
+                      bf16* dd = p.kv + (int64_t)slot * p.kv_slot_stride + (int64_t)l * p.kv_layer_stride + ((int64_t)kh * p.max_len + pos) * HD;
                       const bf16 z0 = __float2bfloat16_rn(y0), z1 = __float2bfloat16_rn(y1);
                       dd[i] = z0;
-                      dd[i + 64] = z1;
-                      st_tag(t_kn + kh * 128 + i, __bfloat162float(z0), tag);      // the cache row as this launch's attention reads it
-                      st_tag(t_kn + kh * 128 + i + 64, __bfloat162float(z1), tag);
+                      dd[i + HALF] = z1;
+                      st_tag(t_kn + kh * HD + i, __bfloat162float(z0), tag);      // the cache row as this launch's attention reads it
+                      st_tag(t_kn + kh * HD + i + HALF, __bfloat162float(z1), tag);
                     }
                   } else {
-                    const int kh = (row0 - qd - kd) >> 7;
-                    bf16* dd = p.kv + (int64_t)slot * p.kv_slot_stride + (int64_t)l * p.kv_layer_stride + p.kv_v_offset + ((int64_t)kh * p.max_len + pos) * 128;
+                    const int kh = (row0 - qd - kd) >> HSH;
+                    bf16* dd = p.kv + (int64_t)slot * p.kv_slot_stride + (int64_t)l * p.kv_layer_stride + p.kv_v_offset + ((int64_t)kh * p.max_len + pos) * HD;
                     const bf16 z0 = __float2bfloat16_rn(a0), z1 = __float2bfloat16_rn(a1);
                     dd[i] = z0;
-                    dd[i + 64] = z1;
-                    st_tag(t_vn + kh * 128 + i, __bfloat162float(z0), tag);
-                    st_tag(t_vn + kh * 128 + i + 64, __bfloat162float(z1), tag);
+                    dd[i + HALF] = z1;
+                    st_tag(t_vn + kh * HD + i, __bfloat162float(z0), tag);
+                    st_tag(t_vn + kh * HD + i + HALF, __bfloat162float(z1), tag);
                   }
                 } else if (ph == PH_O || ph == PH_DOWN) {
                   u64* dst = (ph == PH_O) ? t_xa : t_xb;
@@ -916,7 +939,8 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
 
 // ------------------------------------------------------------------ one-time weight re-tiling
 // dst chunk q (16 B) = tile (group, ks) -> [kstep s][matrix m][row r]: rows-half = m & 1, k-half = m >> 1
-__global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int groups,
+// TILE_ROPE: head blocks of hd rows; group gi holds pair rows (i, i + hd/2) for i in 8 consecutive values
+__global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
                                                      int tpg, bf16* __restrict__ dst) {
   const int64_t q = (int64_t)blockIdx.x * 256 + threadIdx.x;
   const int64_t total = (int64_t)groups * tpg * 512;
@@ -928,7 +952,10 @@ __global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ sr
   const int col = ks * 256 + s * 16 + (m >> 1) * 8;
   int row;
   if (mode == TILE_SEQ) row = gi * 16 + ar;
-  else if (mode == TILE_ROPE) row = (gi >> 3) * 128 + ((gi & 7) << 3) + (ar & 7) + (ar >> 3) * 64;
+  else if (mode == TILE_ROPE) {
+    const int gph = hd / 16;   // groups per head block
+    row = (gi / gph) * hd + ((gi % gph) << 3) + (ar & 7) + (ar >> 3) * (hd / 2);
+  }
   else row = (ar < 8) ? 2 * (gi * 8 + ar) : 2 * (gi * 8 + ar - 8) + 1;  // source rows are interleaved (gate, up)
   uint4 v = make_uint4(0, 0, 0, 0);
   if (row < N && col < K) v = *reinterpret_cast<const uint4*>(src + (int64_t)row * K + col);
@@ -945,24 +972,30 @@ int64_t mega_tiled_elems(int N, int K, int mode, int* groups, int* tpg) {
   return (int64_t)g * t * MEGA_TILE_ELEMS;
 }
 
-cudaError_t launch_retile(const bf16* src, int N, int K, int mode, bf16* dst, cudaStream_t s) {
-  if ((K & 7) || (mode == TILE_ROPE && (N & 127))) return cudaErrorInvalidValue;
+cudaError_t launch_retile(const bf16* src, int N, int K, int mode, int hd, bf16* dst, cudaStream_t s) {
+  if ((K & 7) || (mode == TILE_ROPE && ((hd != 64 && hd != 128) || N % hd))) return cudaErrorInvalidValue;
   int groups, tpg;
   mega_tiled_elems(N, K, mode, &groups, &tpg);
   const int64_t chunks = (int64_t)groups * tpg * 512;
-  retile_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(src, N, K, mode, groups, tpg, dst);
+  retile_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(src, N, K, mode, hd, groups, tpg, dst);
   return cudaGetLastError();
 }
 
+// fixed-size shared memory after the ring and the activation vector: barriers, red, rope_s, tpart, gcnt, rbuf, qkn, slice
+// tables (sized for head_dim 128; head_dim 64 uses a prefix of rope_s and qkn)
 int mega_smem_bytes(const MegaArgs& a) {
   return a.nslots * TILE_BYTES + a.act_floats * 4 + 2 * a.nslots * 8 + (16 + 128 + NT * 16) * 4 + NG * 4 + NG * 16 * 4 + 384 * 4 + NS * 8;
 }
 
-cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int max_smem_optin, int num_sms, int* grid_out) {
+cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int hd, int max_smem_optin, int num_sms, int* grid_out) {
+  if (hd != 64 && hd != 128) return cudaErrorInvalidValue;
+  a.hd = hd;
   auto pad = [](int k) { return (k + 255) / 256 * 256; };
   int actf = pad(H) > pad(I) ? pad(H) : pad(I);
-  if (pad(heads * 128) > actf) actf = pad(heads * 128);
-  if (actf < 32 + 16 * 128 + 16 * 132) actf = 32 + 16 * 128 + 16 * 132;  // attention merge scratch (half-warp states + the head's partials)
+  if (pad(heads * hd) > actf) actf = pad(heads * hd);
+  // attention merge scratch: key-group states (m, l, o) + the head's per-CTA partials (up to 16 records of hd + 4)
+  const int nst = NCW * (256 / hd), merge = 2 * nst + nst * hd + 16 * (hd + 4);
+  if (actf < merge) actf = merge;
   actf = (actf + 31) & ~31;
   a.act_floats = actf;
   a.tg_H = pad(H);
@@ -985,7 +1018,10 @@ cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int max_smem_op
 cudaError_t launch_decode_mega(const MegaArgs& a, int grid, cudaStream_t s, uint64_t* counter) {
   const int smem = mega_smem_bytes(a);
   const bool dbgk = a.dbg != nullptr || a.dbg2 != nullptr || a.dbg_flags != 0;
-  const void* fn = dbgk ? (const void*)decode_mega_kernel<true> : (const void*)decode_mega_kernel<false>;
+  const void* fn;
+  if (a.hd == 128) fn = dbgk ? (const void*)decode_mega_kernel<true, 128> : (const void*)decode_mega_kernel<false, 128>;
+  else if (a.hd == 64) fn = dbgk ? (const void*)decode_mega_kernel<true, 64> : (const void*)decode_mega_kernel<false, 64>;
+  else return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   void* args[] = {(void*)&a};

@@ -81,7 +81,8 @@ std::vector<WEntry> build_table(const dtk_config& c) {
 bool config_ok(const dtk_config& c, std::string& why) {
   auto bad = [&](const char* m) { why = m; return false; };
   if (c.hidden <= 0 || c.inter <= 0 || c.layers <= 0 || c.heads <= 0 || c.kv_heads <= 0 || c.vocab <= 0) return bad("non-positive decoder dims");
-  if (c.head_dim != 128) return bad("decoder head_dim must be 128");
+  if (c.head_dim != 128 && c.head_dim != 64) return bad("decoder head_dim must be 64 or 128");
+  if (c.heads * c.head_dim != c.hidden) return bad("decoder heads * head_dim must equal hidden");
   if (c.heads % c.kv_heads) return bad("heads % kv_heads != 0");
   if ((c.hidden & 7) || (c.inter & 7)) return bad("hidden/inter must be multiples of 8");
   if (c.rope_type != 0 && c.rope_type != 1) return bad("rope_type must be 0 (linear) or 1 (llama3)");
@@ -190,14 +191,14 @@ struct dtk_engine {
   const uint8_t* arena = nullptr;
   std::map<std::string, const bf16*> w;
 
-  // KV slots: [slot][layer][2][kv_head][max_len][128] bf16
+  // KV slots: [slot][layer][2][kv_head][max_len][head_dim] bf16
   bf16* kv = nullptr;
   int64_t kv_layer_stride = 0, kv_v_offset = 0, kv_slot_stride = 0;
   std::vector<char> slot_used;
   // one-level shared KV prefix: positions [0, share_len[s]) of slot s are read from slot share_base[s] (a multiple of 16
   // positions, never written through s); refcnt[b] = sequences borrowing from b, shared_upto[b] = longest prefix lent out
   std::vector<int> share_base, share_len, refcnt, shared_upto;
-  float* rope_cs = nullptr;  // [max_len, 64, 2]
+  float* rope_cs = nullptr;  // [max_len, head_dim/2, 2]
 
   // prefill workspace (max_len rows)
   float *p_x = nullptr, *p_qkv = nullptr;
@@ -560,7 +561,8 @@ int nsplit_for(const dtk_config& c, int B) {
 // one decode step for the B sequences whose (slot, pos, tok) live in d_slots / d_pos / d_tok (or tok64)
 int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits, cudaStream_t s) {
   const dtk_config& c = eng->cfg;
-  const int H = c.hidden, I = c.inter, qd = c.heads * 128, kd = c.kv_heads * 128;
+  const int H = c.hidden, I = c.inter, HD = c.head_dim, qd = c.heads * HD, kd = c.kv_heads * HD;
+  const float scale = 1.0f / sqrtf((float)HD);
   uint64_t* lc = &eng->launches;
   if (B == 1 && eng->decode_impl == 1 && eng->mega_ok) {
     if (tok64) {
@@ -612,15 +614,15 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
       DTK_CK(launch_rmsnorm(eng->d_x, H, W(eng, LN("dec.L", l, "norm1")), c.rms_eps, B, H, eng->p_xn, s, lc));
       DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wqkv")), qkvd, nullptr, 0, eng->p_qkv, nullptr, qkvd));
       DTK_CK(launch_rope_kv_decode(eng->p_qkv, B, eng->d_slots, eng->d_pos, c.heads, c.kv_heads, eng->rope_cs, eng->d_q,
-                                   kv_layer(eng, 0, l), eng->kv_slot_stride, eng->kv_v_offset, c.max_len, s, lc, cas ? eng->p_q : nullptr));
+                                   kv_layer(eng, 0, l), eng->kv_slot_stride, eng->kv_v_offset, c.max_len, HD, s, lc, cas ? eng->p_q : nullptr));
       if (cas) {
         AttnArgs f{};
         f.q = eng->p_q; f.k = kv_layer(eng, eng->cas_slot, l); f.v = f.k + eng->kv_v_offset;
-        f.q_bs = 0; f.q_hs = 128; f.q_rs = qd;
-        f.k_bs = 0; f.k_hs = (int64_t)c.max_len * 128; f.k_rs = 128;
-        f.v_bs = 0; f.v_hs = (int64_t)c.max_len * 128; f.v_rs = 128;
+        f.q_bs = 0; f.q_hs = HD; f.q_rs = qd;
+        f.k_bs = 0; f.k_hs = (int64_t)c.max_len * HD; f.k_rs = HD;
+        f.v_bs = 0; f.v_hs = (int64_t)c.max_len * HD; f.v_rs = HD;
         f.B = 1; f.heads = c.heads; f.kv_group = c.heads / c.kv_heads; f.Tq = B; f.Tk = eng->cas_len; f.q_pos0 = 0;
-        f.causal = 0; f.head_dim = 128; f.scale = 1.0f / sqrtf(128.f);
+        f.causal = 0; f.head_dim = HD; f.scale = scale;
         f.part_o = eng->d_part_o; f.part_ml = eng->d_part_ml; f.part_np = nsplit + csplit; f.part_idx0 = nsplit; f.part_tiles = ctile;
         DTK_CK(launch_flash_attn(f, s, lc));
       }
@@ -629,7 +631,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
         a.q = eng->d_q; a.q_stride = qd; a.kv_base = kv_layer(eng, 0, l); a.kv_slot_stride = eng->kv_slot_stride;
         a.kv_v_offset = eng->kv_v_offset; a.slots = eng->d_slots; a.pos = eng->d_pos; a.share_slot = eng->d_share_slot; a.share_len = eng->d_share_len;
         a.B = B; a.heads = c.heads; a.kv_group = c.heads / c.kv_heads; a.max_len = c.max_len; a.nsplit = nsplit;
-        a.scale = 1.0f / sqrtf(128.f);
+        a.head_dim = HD; a.scale = scale;
         a.part_o = eng->d_part_o; a.part_ml = eng->d_part_ml; a.counters = eng->d_counters;
         a.out = eng->d_att; a.out_stride = qd; a.out_bf16 = eng->p_att;   // bf16 copy = the o-proj operand (no cast launch)
         if (cas) { a.key_begin = eng->cas_len; a.np = nsplit + csplit; }
@@ -652,7 +654,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
       g.out = eng->d_q; g.out_stride = qd; g.B = B;
       g.slots = eng->d_slots; g.pos = eng->d_pos; g.rope_cs = eng->rope_cs;
       g.kv_base = kv_layer(eng, 0, l); g.kv_slot_stride = eng->kv_slot_stride; g.kv_v_offset = eng->kv_v_offset;
-      g.q_dim = qd; g.kv_dim = kd; g.max_len = c.max_len;
+      g.q_dim = qd; g.kv_dim = kd; g.max_len = c.max_len; g.head_dim = HD;
       DTK_CK(launch_gemv(g, s, lc));
     }
     {
@@ -660,7 +662,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
       a.q = eng->d_q; a.q_stride = qd; a.kv_base = kv_layer(eng, 0, l); a.kv_slot_stride = eng->kv_slot_stride;
       a.kv_v_offset = eng->kv_v_offset; a.slots = eng->d_slots; a.pos = eng->d_pos; a.share_slot = eng->d_share_slot; a.share_len = eng->d_share_len;
       a.B = B; a.heads = c.heads; a.kv_group = c.heads / c.kv_heads; a.max_len = c.max_len; a.nsplit = nsplit;
-      a.scale = 1.0f / sqrtf(128.f);
+      a.head_dim = HD; a.scale = scale;
       a.part_o = eng->d_part_o; a.part_ml = eng->d_part_ml; a.counters = eng->d_counters;
       a.out = eng->d_att; a.out_stride = qd;
       DTK_CK(launch_decode_attn(a, s, lc));
@@ -762,8 +764,8 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
   for (auto& e : build_table(*cfg)) eng->w[e.name] = (const bf16*)(eng->arena + e.offset);
 
   const dtk_config& c = eng->cfg;
-  const int64_t H = c.hidden, I = c.inter, V = c.vocab, qd = c.heads * 128, kd = c.kv_heads * 128, T = c.max_len, MB = c.max_batch;
-  eng->kv_v_offset = (int64_t)c.kv_heads * c.max_len * 128;
+  const int64_t HD = c.head_dim, H = c.hidden, I = c.inter, V = c.vocab, qd = c.heads * HD, kd = c.kv_heads * HD, T = c.max_len, MB = c.max_batch;
+  eng->kv_v_offset = (int64_t)c.kv_heads * c.max_len * HD;
   eng->kv_layer_stride = 2 * eng->kv_v_offset;
   eng->kv_slot_stride = eng->kv_layer_stride * c.layers;
   DTK_ALLOC(eng->kv, eng->kv_slot_stride * c.max_seqs);
@@ -775,7 +777,7 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
 
   {
     std::vector<float> tab = rope_table(c.rope_theta, c.rope_factor, c.rope_type, c.rope_low_freq, c.rope_high_freq,
-                                        c.rope_orig_max_pos, 128, T);
+                                        c.rope_orig_max_pos, (int)HD, T);
     DTK_ALLOC(eng->rope_cs, tab.size());
     DTK_CK(cudaMemcpy(eng->rope_cs, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
@@ -791,7 +793,7 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
   DTK_ALLOC(eng->d_h, MB * I);
   DTK_ALLOC(eng->d_logits, MB * V);
   DTK_ALLOC(eng->d_scratch, MB * V);
-  DTK_ALLOC(eng->d_part_o, MB * c.heads * 16 * 128);
+  DTK_ALLOC(eng->d_part_o, MB * c.heads * 16 * HD);
   DTK_ALLOC(eng->d_part_ml, MB * c.heads * 16 * 2);
   DTK_ALLOC(eng->d_counters, MB * c.heads + 1);
   DTK_CK(cudaMemset(eng->d_counters, 0, (MB * c.heads + 1) * sizeof(unsigned int)));
@@ -812,16 +814,16 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
     DTK_CK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
     MegaArgs& m = eng->mega;
     int grid = 0;
-    if (coop && mega_configure(m, c.hidden, c.inter, c.heads, smem_optin, sms, &grid) == cudaSuccess) {
+    if (coop && mega_configure(m, c.hidden, c.inter, c.heads, c.head_dim, smem_optin, sms, &grid) == cudaSuccess) {
       m.H = c.hidden; m.I = c.inter; m.L = c.layers; m.heads = c.heads; m.kv_heads = c.kv_heads; m.V = c.vocab;
       m.max_len = c.max_len; m.eps = c.rms_eps;
       m.embed = W(eng, "dec.embed"); m.final_norm = W(eng, "dec.norm");
       m.norm1_0 = W(eng, "dec.L0.norm1"); m.norm2_0 = W(eng, "dec.L0.norm2");
       m.norm_stride = c.layers > 1 ? (int64_t)(W(eng, "dec.L1.norm1") - W(eng, "dec.L0.norm1")) : 0;
       // decode-side tiled weight copy (one-time, on device): [layer][qkv | o | gu | down] ... [lm_head]
-      const int qkvN = (c.heads + 2 * c.kv_heads) * 128, qd = c.heads * 128;
+      const int qkvN = (int)((c.heads + 2 * c.kv_heads) * HD);
       struct Spec { MegaMat* mm; const char* name; int N, K, mode; } specs[4] = {
-          {&m.mat[0], "wqkv", qkvN, c.hidden, TILE_ROPE}, {&m.mat[1], "wo", c.hidden, qd, TILE_SEQ},
+          {&m.mat[0], "wqkv", qkvN, c.hidden, TILE_ROPE}, {&m.mat[1], "wo", c.hidden, (int)qd, TILE_SEQ},
           {&m.mat[2], "wgu", 2 * c.inter, c.hidden, TILE_GLU}, {&m.mat[3], "wd", c.hidden, c.inter, TILE_SEQ}};
       int64_t per_layer = 0, off[4];
       for (int i = 0; i < 4; ++i) {
@@ -834,7 +836,7 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
         MegaMat& mm = *specs[i].mm;
         mm.base = eng->d_tiled + off[i]; mm.layer_stride = per_layer; mm.N = specs[i].N; mm.K = specs[i].K; mm.mode = specs[i].mode;
         for (int l = 0; l < c.layers; ++l)
-          DTK_CK(launch_retile(W(eng, LN("dec.L", l, specs[i].name)), specs[i].N, specs[i].K, specs[i].mode,
+          DTK_CK(launch_retile(W(eng, LN("dec.L", l, specs[i].name)), specs[i].N, specs[i].K, specs[i].mode, c.head_dim,
                                eng->d_tiled + (int64_t)l * per_layer + off[i], 0));
       }
       for (int i = 0; i < 5; ++i) {
@@ -842,13 +844,13 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
         m.mat[i].nact = (m.mat[i].groups + m.mat[i].per - 1) / m.mat[i].per;
       }
       m.mat[4].base = eng->d_tiled + per_layer * c.layers; m.mat[4].layer_stride = 0; m.mat[4].N = c.vocab; m.mat[4].K = c.hidden; m.mat[4].mode = TILE_SEQ;
-      DTK_CK(launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, eng->d_tiled + per_layer * c.layers, 0));
+      DTK_CK(launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, c.head_dim, eng->d_tiled + per_layer * c.layers, 0));
       m.tok = eng->d_tok; m.pos = eng->d_pos; m.slots = eng->d_slots; m.share_slot = eng->d_share_slot; m.share_len = eng->d_share_len;
       m.kv = eng->kv; m.kv_slot_stride = eng->kv_slot_stride; m.kv_layer_stride = eng->kv_layer_stride;
       m.kv_v_offset = eng->kv_v_offset; m.rope_cs = eng->rope_cs;
       m.logits = eng->d_logits;
       {
-        const int64_t words = 2 * (int64_t)m.tg_H + 2 * (int64_t)qd + 2 * (int64_t)c.kv_heads * 128 + m.tg_I + (int64_t)grid * 132;
+        const int64_t words = 2 * (int64_t)m.tg_H + 2 * qd + 2 * kd + m.tg_I + (int64_t)grid * (HD + 4);
         DTK_ALLOC(eng->d_tagged, words);
         DTK_CK(cudaMemset(eng->d_tagged, 0, (size_t)words * sizeof(unsigned long long)));
         m.tg = eng->d_tagged;
@@ -1146,9 +1148,10 @@ namespace {
 int copy_kv_range(dtk_engine* eng, int src, int dst, int p0, int p1, cudaStream_t s) {
   if (p1 <= p0) return DTK_OK;
   const dtk_config& c = eng->cfg;
-  const size_t pitch = (size_t)c.max_len * 128 * sizeof(bf16);
-  DTK_CK(cudaMemcpy2DAsync(kv_layer(eng, dst, 0) + (int64_t)p0 * 128, pitch, kv_layer(eng, src, 0) + (int64_t)p0 * 128, pitch,
-                           (size_t)(p1 - p0) * 128 * sizeof(bf16), (size_t)c.layers * 2 * c.kv_heads, cudaMemcpyDeviceToDevice, s));
+  const int64_t HD = c.head_dim;
+  const size_t pitch = (size_t)c.max_len * HD * sizeof(bf16);
+  DTK_CK(cudaMemcpy2DAsync(kv_layer(eng, dst, 0) + p0 * HD, pitch, kv_layer(eng, src, 0) + p0 * HD, pitch,
+                           (size_t)(p1 - p0) * HD * sizeof(bf16), (size_t)c.layers * 2 * c.kv_heads, cudaMemcpyDeviceToDevice, s));
   return DTK_OK;
 }
 void drop_share(dtk_engine* eng, int slot) {
@@ -1240,7 +1243,7 @@ int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_
   DTK_CK(cudaSetDevice(eng->device));
   cudaStream_t s = (cudaStream_t)stream;
   uint64_t* lc = &eng->launches;
-  const int H = c.hidden, I = c.inter, qd = c.heads * 128, kd = c.kv_heads * 128;
+  const int H = c.hidden, I = c.inter, HD = c.head_dim, qd = c.heads * HD, kd = c.kv_heads * HD;
   DTK_CK(launch_embed_splice(ids, T, start_pos, W(eng, "dec.embed"), H, c.vocab, c.image_token_id, img_embeds, img_start,
                              n_img, eng->p_x, s, lc));
   for (int l = 0; l < c.layers; ++l) {
@@ -1253,16 +1256,16 @@ int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_
     }
     bf16* kc = kv_layer(eng, slot, l);
     bf16* vc = kc + eng->kv_v_offset;
-    DTK_CK(launch_rope_kv_prefill(eng->p_qkv, T, start_pos, c.heads, c.kv_heads, eng->rope_cs, eng->p_q, kc, vc, c.max_len, s, lc));
+    DTK_CK(launch_rope_kv_prefill(eng->p_qkv, T, start_pos, c.heads, c.kv_heads, eng->rope_cs, eng->p_q, kc, vc, c.max_len, HD, s, lc));
     {
       AttnArgs a{};
       a.q = eng->p_q; a.k = kc; a.v = vc; a.o = eng->p_att;
-      a.q_bs = 0; a.q_hs = 128; a.q_rs = qd;
-      a.k_bs = 0; a.k_hs = (int64_t)c.max_len * 128; a.k_rs = 128;
-      a.v_bs = 0; a.v_hs = (int64_t)c.max_len * 128; a.v_rs = 128;
-      a.o_bs = 0; a.o_hs = 128; a.o_rs = qd;
+      a.q_bs = 0; a.q_hs = HD; a.q_rs = qd;
+      a.k_bs = 0; a.k_hs = (int64_t)c.max_len * HD; a.k_rs = HD;
+      a.v_bs = 0; a.v_hs = (int64_t)c.max_len * HD; a.v_rs = HD;
+      a.o_bs = 0; a.o_hs = HD; a.o_rs = qd;
       a.B = 1; a.heads = c.heads; a.kv_group = c.heads / c.kv_heads; a.Tq = T; a.Tk = start_pos + T; a.q_pos0 = start_pos;
-      a.causal = 1; a.head_dim = 128; a.scale = 1.0f / sqrtf(128.f);
+      a.causal = 1; a.head_dim = HD; a.scale = 1.0f / sqrtf((float)HD);
       if (eng->share_len[slot] > 0) {   // keys below the shared length come from the base slot
         a.k2 = kv_layer(eng, eng->share_base[slot], l);
         a.v2 = a.k2 + eng->kv_v_offset;

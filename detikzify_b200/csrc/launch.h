@@ -54,7 +54,7 @@ struct AttnArgs {
   int Tq, Tk;
   int q_pos0;                 // causal: query i sits at position q_pos0 + i; key j visible iff j <= pos
   int causal;
-  int head_dim;               // 72 or 128
+  int head_dim;               // 72, 64 or 128
   float scale;
   // shared KV prefix (prefill on a sequence that borrows positions [0, split_row) from another slot): key rows below
   // split_row are read from k2 / v2 (same strides), the rest from k / v. split_row = 0: everything from k / v.
@@ -64,7 +64,7 @@ struct AttnArgs {
   // rollouts of one figure, blockIdx.x selects a range of part_tiles key tiles, and instead of the normalised output the
   // kernel exports the flash state of that range in the convention of decode_attn_kernel's partials:
   //   part_ml[(row * heads + head) * part_np + part_idx0 + blockIdx.x] = { max score * scale * log2(e), sum exp2 },
-  //   part_o[... * 128 + d] = unnormalised output.
+  //   part_o[... * head_dim + d] = unnormalised output (head_dim 64 or 128).
   float *part_o, *part_ml;
   int part_np, part_idx0, part_tiles;
 };
@@ -96,13 +96,15 @@ cudaError_t launch_cast_f32_bf16(const float* in, bf16* out, int64_t n, cudaStre
 cudaError_t launch_embed_splice(const int64_t* ids, int T, int start_pos, const bf16* embed, int H, int vocab,
                                 int image_token, const float* img, int img_start, int n_img, float* x,
                                 cudaStream_t s, uint64_t* counter);
-// prefill: qkv fp32 [T, qd+2kd] -> roped q bf16 [T, qd]; K/V bf16 into the cache at positions start_pos+t
+// decoder RoPE + KV append, head_dim hd in {64, 128}; rope_cs fp32 [max_len, hd/2, 2]; cache rows [kv_head][max_len][hd].
+// decode: qkv fp32 [B, qd+2kd] -> roped q fp32 (and optionally bf16) [B, qd]; K/V of row b into slot slots[b] at pos[b]
 cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, int heads, int kv_heads,
                                   const float* rope_cs, float* q_out, bf16* kv_base, int64_t kv_slot_stride,
-                                  int64_t kv_v_offset, int max_len, cudaStream_t s, uint64_t* counter, bf16* q_bf16 = nullptr);
+                                  int64_t kv_v_offset, int max_len, int hd, cudaStream_t s, uint64_t* counter, bf16* q_bf16 = nullptr);
+// prefill: qkv fp32 [T, qd+2kd] -> roped q bf16 [T, qd]; K/V bf16 into the cache at positions start_pos+t
 cudaError_t launch_rope_kv_prefill(const float* qkv, int T, int start_pos, int heads, int kv_heads,
                                    const float* rope_cs, bf16* q_out, bf16* kcache, bf16* vcache,
-                                   int max_len, cudaStream_t s, uint64_t* counter);
+                                   int max_len, int hd, cudaStream_t s, uint64_t* counter);
 // head_dim 64 prefill without a KV slot (caption encoder): qkv fp32 [T, (heads+2kv_heads)*64] -> roped q bf16 [T, heads*64],
 // roped k bf16 [T, kv_heads*64], v bf16 [T, kv_heads*64]; rope_cs fp32 [T, 32, 2]
 cudaError_t launch_rope_qkv64(const float* qkv, int T, int heads, int kv_heads, const float* rope_cs, bf16* q, bf16* k, bf16* v,
@@ -128,11 +130,12 @@ struct GemvArgs {
   // QKV mode
   const int* slots;           // device int[B]
   const int* pos;             // device int[B] : position of the token being processed
-  const float* rope_cs;       // fp32 [max_len, 64, 2] (cos, sin)
+  const float* rope_cs;       // fp32 [max_len, head_dim/2, 2] (cos, sin)
   bf16* kv_base;              // cache base of this layer for slot 0: K then V
   int64_t kv_slot_stride;     // elements between slots
   int64_t kv_v_offset;        // elements from K to V of the same layer
   int q_dim, kv_dim, max_len;
+  int head_dim;               // 64 or 128
 };
 cudaError_t launch_gemv(const GemvArgs& a, cudaStream_t s, uint64_t* counter);
 
@@ -150,8 +153,9 @@ struct DecodeAttnArgs {
   const int* share_slot;      // device int[B]: slot that holds positions [0, share_len[b]) of sequence b (shared prefix)
   const int* share_len;       // device int[B]: 0 = nothing shared
   int B, heads, kv_group, max_len, nsplit;
+  int head_dim;               // 64 or 128
   float scale;
-  float* part_o;              // [B, heads, np, 128]
+  float* part_o;              // [B, heads, np, head_dim]
   float* part_ml;             // [B, heads, np, 2]
   unsigned int* counters;     // [B * heads], zero-initialised, self-resetting
   float* out;                 // [B, q_dim] fp32
@@ -198,7 +202,7 @@ int get_sample_impl();
 // ---------------------------------------------------------------- persistent decode kernel (B = 1)
 // Decode-side weight copy: every matrix is re-tiled once at load into 8 KB tiles of 16 rows x 256 k that a
 // single 1-D bulk copy lands in shared memory exactly as ldmatrix.x4 wants them ([kstep 16][matrix 4][row 8][8 bf16]).
-// Row groups are permuted so that the two accumulator rows (g, g+8) of one thread are a RoPE pair (i, i+64)
+// Row groups are permuted so that the two accumulator rows (g, g+8) of one thread are a RoPE pair (i, i+head_dim/2)
 // or a SwiGLU pair (gate_i, up_i).
 enum { TILE_SEQ = 0, TILE_ROPE = 1, TILE_GLU = 2 };
 constexpr int MEGA_TILE_ELEMS = 4096;  // 16 x 256 bf16 = 8 KB
@@ -213,6 +217,7 @@ struct MegaMat {
 };
 struct MegaArgs {
   int H, I, L, heads, kv_heads, V, max_len;
+  int hd;                                                     // decoder head_dim, 64 or 128 (mega_configure)
   float eps;
   const bf16 *embed, *final_norm;
   const bf16 *norm1_0, *norm2_0;                               // row-major arena; layer l = ptr + l * norm_stride
@@ -224,8 +229,8 @@ struct MegaArgs {
   int64_t kv_slot_stride, kv_layer_stride, kv_v_offset;
   const float* rope_cs;
   float* logits;
-  // tagged cross-CTA activation words {fp32 value, phase tag} (zero-initialised): xa[tg_H] xb[tg_H] q[heads*128]
-  // knew[kv_heads*128] vnew[kv_heads*128] attn[heads*128] h[tg_I] part[grid][132]
+  // tagged cross-CTA activation words {fp32 value, phase tag} (zero-initialised): xa[tg_H] xb[tg_H] q[heads*hd]
+  // knew[kv_heads*hd] vnew[kv_heads*hd] attn[heads*hd] h[tg_I] part[grid][hd+4]
   unsigned long long* tg;
   int tg_H, tg_I;                                             // H and I padded to the 256-column tile (mega_configure)
   unsigned int* head_cnt;                                     // [heads] arrival counters (zero-initialised, self-resetting)
@@ -243,11 +248,11 @@ struct MegaArgs {
   int dbg_layer;
 };
 int mega_smem_bytes(const MegaArgs& a);
-cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int max_smem_optin, int num_sms, int* grid_out);
+cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int hd, int max_smem_optin, int num_sms, int* grid_out);
 cudaError_t launch_decode_mega(const MegaArgs& a, int grid, cudaStream_t s, uint64_t* counter);
-// one-time re-tiling of a row-major [N, K] (ld = K) matrix into the decode layout
+// one-time re-tiling of a row-major [N, K] (ld = K) matrix into the decode layout (hd: head_dim of TILE_ROPE)
 int64_t mega_tiled_elems(int N, int K, int mode, int* groups, int* tpg);
-cudaError_t launch_retile(const bf16* src, int N, int K, int mode, bf16* dst, cudaStream_t s);
+cudaError_t launch_retile(const bf16* src, int N, int K, int mode, int hd, bf16* dst, cudaStream_t s);
 
 // device image preprocessing (Pillow-exact 8-bit bicubic resize + rescale + normalise): rgb uint8 [h, w, 3] -> fp32 [3, S, S]
 cudaError_t launch_image_preprocess(const uint8_t* rgb, int h, int w, int S, const int* bounds_h, const int* coef_h, int ksize_h,

@@ -190,30 +190,32 @@ __global__ void __launch_bounds__(128) embed_splice_kernel(const int64_t* __rest
 }
 
 // ---- prefill RoPE + KV-cache write (HF modeling_llama.py:124-168 rotate-half; cache append :269-270).
-//      grid (T, heads + 2*kv_heads); 64 threads: thread i handles the pair (i, i+64).
-__global__ void __launch_bounds__(64) rope_kv_prefill_kernel(const float* __restrict__ qkv, int T, int start_pos,
-                                                             int heads, int kv_heads,
-                                                             const float* __restrict__ rope_cs,
-                                                             bf16* __restrict__ q_out, bf16* __restrict__ kcache,
-                                                             bf16* __restrict__ vcache, int max_len) {
+//      grid (T, heads + 2*kv_heads); HD/2 threads: thread i handles the pair (i, i+HD/2).
+template <int HD>
+__global__ void __launch_bounds__(HD / 2) rope_kv_prefill_kernel(const float* __restrict__ qkv, int T, int start_pos,
+                                                                 int heads, int kv_heads,
+                                                                 const float* __restrict__ rope_cs,
+                                                                 bf16* __restrict__ q_out, bf16* __restrict__ kcache,
+                                                                 bf16* __restrict__ vcache, int max_len) {
+  constexpr int HALF = HD / 2;
   const int t = blockIdx.x, hh = blockIdx.y, i = threadIdx.x;
-  const int qd = heads * 128, kd = kv_heads * 128;
+  const int qd = heads * HD, kd = kv_heads * HD;
   const int pos = start_pos + t;
-  const float* src = qkv + (int64_t)t * (qd + 2 * kd) + hh * 128;
-  const float a = src[i], b = src[i + 64];
-  const float2 cs = *reinterpret_cast<const float2*>(rope_cs + ((int64_t)pos * 64 + i) * 2);
+  const float* src = qkv + (int64_t)t * (qd + 2 * kd) + hh * HD;
+  const float a = src[i], b = src[i + HALF];
+  const float2 cs = *reinterpret_cast<const float2*>(rope_cs + ((int64_t)pos * HALF + i) * 2);
   if (hh < heads) {
-    bf16* d = q_out + (int64_t)t * qd + hh * 128;
+    bf16* d = q_out + (int64_t)t * qd + hh * HD;
     d[i] = __float2bfloat16_rn(a * cs.x - b * cs.y);
-    d[i + 64] = __float2bfloat16_rn(b * cs.x + a * cs.y);
+    d[i + HALF] = __float2bfloat16_rn(b * cs.x + a * cs.y);
   } else if (hh < heads + kv_heads) {
-    bf16* d = kcache + ((int64_t)(hh - heads) * max_len + pos) * 128;
+    bf16* d = kcache + ((int64_t)(hh - heads) * max_len + pos) * HD;
     d[i] = __float2bfloat16_rn(a * cs.x - b * cs.y);
-    d[i + 64] = __float2bfloat16_rn(b * cs.x + a * cs.y);
+    d[i + HALF] = __float2bfloat16_rn(b * cs.x + a * cs.y);
   } else {
-    bf16* d = vcache + ((int64_t)(hh - heads - kv_heads) * max_len + pos) * 128;
+    bf16* d = vcache + ((int64_t)(hh - heads - kv_heads) * max_len + pos) * HD;
     d[i] = __float2bfloat16_rn(a);
-    d[i + 64] = __float2bfloat16_rn(b);
+    d[i + HALF] = __float2bfloat16_rn(b);
   }
 }
 
@@ -288,35 +290,37 @@ __global__ void __launch_bounds__(256) cast_bf16_f32_kernel(const bf16* __restri
 
 // ---- batched-decode RoPE + KV-cache append: row b belongs to sequence slots[b] at position pos[b]
 //      (HF modeling_llama.py:124-168; DynamicCache.update). grid (B, heads + 2*kv_heads); 64 threads.
-__global__ void __launch_bounds__(64) rope_kv_decode_kernel(const float* __restrict__ qkv, const int* __restrict__ slots,
-                                                            const int* __restrict__ posv, int heads, int kv_heads,
-                                                            const float* __restrict__ rope_cs, float* __restrict__ q_out,
-                                                            bf16* __restrict__ kv_base, int64_t kv_slot_stride,
-                                                            int64_t kv_v_offset, int max_len, bf16* __restrict__ q_bf16) {
+template <int HD>
+__global__ void __launch_bounds__(HD / 2) rope_kv_decode_kernel(const float* __restrict__ qkv, const int* __restrict__ slots,
+                                                                const int* __restrict__ posv, int heads, int kv_heads,
+                                                                const float* __restrict__ rope_cs, float* __restrict__ q_out,
+                                                                bf16* __restrict__ kv_base, int64_t kv_slot_stride,
+                                                                int64_t kv_v_offset, int max_len, bf16* __restrict__ q_bf16) {
+  constexpr int HALF = HD / 2;
   const int b = blockIdx.x, hh = blockIdx.y, i = threadIdx.x;
-  const int qd = heads * 128, kd = kv_heads * 128;
+  const int qd = heads * HD, kd = kv_heads * HD;
   const int pos = posv[b];
-  const float* src = qkv + (int64_t)b * (qd + 2 * kd) + hh * 128;
-  const float a = src[i], c = src[i + 64];
-  const float2 cs = *reinterpret_cast<const float2*>(rope_cs + ((int64_t)pos * 64 + i) * 2);
+  const float* src = qkv + (int64_t)b * (qd + 2 * kd) + hh * HD;
+  const float a = src[i], c = src[i + HALF];
+  const float2 cs = *reinterpret_cast<const float2*>(rope_cs + ((int64_t)pos * HALF + i) * 2);
   if (hh < heads) {
-    float* d = q_out + (int64_t)b * qd + hh * 128;
+    float* d = q_out + (int64_t)b * qd + hh * HD;
     const float y0 = a * cs.x - c * cs.y, y1 = c * cs.x + a * cs.y;
     d[i] = y0;
-    d[i + 64] = y1;
+    d[i + HALF] = y1;
     if (q_bf16) {   // operand of the shared-prefix attention (tensor cores)
-      bf16* d16 = q_bf16 + (int64_t)b * qd + hh * 128;
+      bf16* d16 = q_bf16 + (int64_t)b * qd + hh * HD;
       d16[i] = __float2bfloat16_rn(y0);
-      d16[i + 64] = __float2bfloat16_rn(y1);
+      d16[i + HALF] = __float2bfloat16_rn(y1);
     }
   } else if (hh < heads + kv_heads) {
-    bf16* d = kv_base + (int64_t)slots[b] * kv_slot_stride + ((int64_t)(hh - heads) * max_len + pos) * 128;
+    bf16* d = kv_base + (int64_t)slots[b] * kv_slot_stride + ((int64_t)(hh - heads) * max_len + pos) * HD;
     d[i] = __float2bfloat16_rn(a * cs.x - c * cs.y);
-    d[i + 64] = __float2bfloat16_rn(c * cs.x + a * cs.y);
+    d[i + HALF] = __float2bfloat16_rn(c * cs.x + a * cs.y);
   } else {
-    bf16* d = kv_base + (int64_t)slots[b] * kv_slot_stride + kv_v_offset + ((int64_t)(hh - heads - kv_heads) * max_len + pos) * 128;
+    bf16* d = kv_base + (int64_t)slots[b] * kv_slot_stride + kv_v_offset + ((int64_t)(hh - heads - kv_heads) * max_len + pos) * HD;
     d[i] = __float2bfloat16_rn(a);
-    d[i + 64] = __float2bfloat16_rn(c);
+    d[i + HALF] = __float2bfloat16_rn(c);
   }
 }
 
@@ -408,11 +412,12 @@ cudaError_t launch_embed_splice(const int64_t* ids, int T, int start_pos, const 
   return cudaGetLastError();
 }
 cudaError_t launch_rope_kv_prefill(const float* qkv, int T, int start_pos, int heads, int kv_heads,
-                                   const float* rope_cs, bf16* q_out, bf16* kcache, bf16* vcache, int max_len,
+                                   const float* rope_cs, bf16* q_out, bf16* kcache, bf16* vcache, int max_len, int hd,
                                    cudaStream_t s, uint64_t* counter) {
   dim3 grid(T, heads + 2 * kv_heads);
-  rope_kv_prefill_kernel<<<grid, 64, 0, s>>>(qkv, T, start_pos, heads, kv_heads, rope_cs, q_out, kcache, vcache,
-                                             max_len);
+  if (hd == 128) rope_kv_prefill_kernel<128><<<grid, 64, 0, s>>>(qkv, T, start_pos, heads, kv_heads, rope_cs, q_out, kcache, vcache, max_len);
+  else if (hd == 64) rope_kv_prefill_kernel<64><<<grid, 32, 0, s>>>(qkv, T, start_pos, heads, kv_heads, rope_cs, q_out, kcache, vcache, max_len);
+  else return cudaErrorInvalidValue;
   if (counter) ++*counter;
   return cudaGetLastError();
 }
@@ -437,10 +442,15 @@ cudaError_t launch_cast_bf16_f32(const bf16* in, float* out, int64_t n, cudaStre
 }
 cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, int heads, int kv_heads,
                                   const float* rope_cs, float* q_out, bf16* kv_base, int64_t kv_slot_stride,
-                                  int64_t kv_v_offset, int max_len, cudaStream_t s, uint64_t* counter, bf16* q_bf16) {
+                                  int64_t kv_v_offset, int max_len, int hd, cudaStream_t s, uint64_t* counter, bf16* q_bf16) {
   dim3 grid(B, heads + 2 * kv_heads);
-  rope_kv_decode_kernel<<<grid, 64, 0, s>>>(qkv, slots, pos, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
-                                            kv_v_offset, max_len, q_bf16);
+  if (hd == 128)
+    rope_kv_decode_kernel<128><<<grid, 64, 0, s>>>(qkv, slots, pos, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
+                                                   kv_v_offset, max_len, q_bf16);
+  else if (hd == 64)
+    rope_kv_decode_kernel<64><<<grid, 32, 0, s>>>(qkv, slots, pos, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
+                                                  kv_v_offset, max_len, q_bf16);
+  else return cudaErrorInvalidValue;
   if (counter) ++*counter;
   return cudaGetLastError();
 }

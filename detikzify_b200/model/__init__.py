@@ -25,12 +25,12 @@ from .modeling import DetikzifyForCausalLM
 from .processing import DetikzifyImageProcessor, DetikzifyProcessor, SyntheticTokenizer
 from .weights import canonical_shapes, convert_timm_vision, convert_v2_state_dict, random_init
 
-# v1 checkpoints with a shape preset. The reference also lists detikzify-tl-1.1b (TinyLlama: head_dim 64, which the decode
-# kernels do not support) and detikzify-cl-7b (no offline config to derive a preset from); a local directory of either loads
-# through its config.json and fails loudly at engine creation if the shape is unsupported.
+# the v1 checkpoints the reference lists (reference detikzify/model/v1/__init__.py:10-15), each with a shape preset
 v1_models = [
     "nllg/detikzify-ds-1.3b",
     "nllg/detikzify-ds-7b",
+    "nllg/detikzify-tl-1.1b",
+    "nllg/detikzify-cl-7b",
 ]
 
 

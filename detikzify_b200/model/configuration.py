@@ -10,8 +10,10 @@ Mirrors the attribute names the reference's callers read:
   * ``config.num_patches`` / ``concat_patches`` / ``feature_layer`` / ``mm_hidden_size``
     (detikzify/model/v1/modeling_detikzify.py:98-107).
 
-Decoder dims of the named checkpoints are the public DeepSeek-Coder base configs
-(SURVEY.md Appendix A); they are config input, not reference source.
+Decoder dims of the named checkpoints are the public DeepSeek-Coder, TinyLlama-1.1B and CodeLlama-7b base configs
+(SURVEY.md Appendix A); they are config input, not reference source. The tl-1.1b / cl-7b vocab sizes follow the v1
+loader's rule (add ``<pad>``, resize to a multiple of 8: reference v1/__init__.py:43-44) and are unverified against
+the hub; a checkpoint directory's ``config.json`` always wins.
 """
 from __future__ import annotations
 
@@ -126,6 +128,32 @@ def preset(name: str) -> DetikzifyConfig:
                                num_attention_heads=32, num_key_value_heads=32, name_or_path=name,
                                vision_config=VisionConfig(hidden_size=144, intermediate_size=176, num_hidden_layers=2,
                                                           num_attention_heads=2, image_size=56, patch_size=14))
+    if key in ("detikzify-tl-1.1b", "tl-1.1b"):
+        # TinyLlama-1.1B: head_dim 64, GQA 32/4; V = 32000 + <pad> -> 32008; patch token = BOS (v1/__init__.py:49)
+        return DetikzifyConfig(hidden_size=2048, intermediate_size=5632, num_hidden_layers=22, num_attention_heads=32,
+                               num_key_value_heads=4, head_dim=64, vocab_size=32008, max_position_embeddings=2048,
+                               rms_norm_eps=1e-5, rope_theta=10000.0, rope_factor=1.0,
+                               bos_token_id=1, eos_token_id=2, pad_token_id=32000, patch_token_id=1, name_or_path=name)
+    if key in ("detikzify-cl-7b", "cl-7b", "detikzify-cl-7b-2l", "cl-7b-2l"):
+        # CodeLlama-7b: MHA 32 x 128, theta 1e6; V = 32016 + <pad> -> 32024. "-2l": parity-test shape (two decoder layers,
+        # small tower) with every cl-7b matrix shape
+        two = key.endswith("-2l")
+        return DetikzifyConfig(hidden_size=4096, intermediate_size=11008, num_hidden_layers=2 if two else 32,
+                               num_attention_heads=32, num_key_value_heads=32, vocab_size=32024, max_position_embeddings=16384,
+                               rms_norm_eps=1e-5, rope_theta=1000000.0, rope_factor=1.0,
+                               bos_token_id=1, eos_token_id=2, pad_token_id=32016, patch_token_id=1, name_or_path=name,
+                               vision_config=VisionConfig(hidden_size=144, intermediate_size=176, num_hidden_layers=2,
+                                                          num_attention_heads=2, image_size=56, patch_size=14)
+                               if two else VisionConfig())
+    if key == "tiny-tl":   # TinyLlama wiring at a CPU-test size: head_dim 64, GQA 8/1, V = 520 (8 mod 16), no RoPE scaling
+        return DetikzifyConfig(
+            hidden_size=512, intermediate_size=1408, num_hidden_layers=2, num_attention_heads=8,
+            num_key_value_heads=1, head_dim=64, vocab_size=520, model_max_length=128, max_position_embeddings=2048,
+            rms_norm_eps=1e-5, rope_theta=10000.0, rope_factor=1.0,
+            bos_token_id=500, eos_token_id=501, pad_token_id=502, patch_token_id=500,
+            name_or_path=name,
+            vision_config=VisionConfig(hidden_size=144, intermediate_size=176, num_hidden_layers=2,
+                                       num_attention_heads=2, image_size=56, patch_size=14))
     if key in ("detikzify-v2-8b", "detikzify-v2.5-8b", "v2-8b", "v2.5-8b"):
         # v2 / v2.5 (reference detikzify/model/configuration_detikzify.py:31-58,83-120, modeling_detikzify.py:62-86): SigLIP
         # so400m at 420 px -> 900 patches -> 300 image tokens, bias-free connector, LLaMA-3.1-8B decoder (GQA 32/8,

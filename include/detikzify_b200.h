@@ -45,7 +45,7 @@ typedef enum dtk_status {
 /* Model shape. Mirrors LlamaConfig / timm-SigLIP dims the reference loads
  * (detikzify/model/v1/configuration_detikzify.py:3-13, SURVEY.md Appendix A). */
 typedef struct dtk_config {
-  /* decoder */
+  /* decoder; head_dim 64 or 128 with heads * head_dim == hidden */
   int32_t hidden, inter, layers, heads, kv_heads, head_dim, vocab, max_len;
   float rms_eps, rope_theta, rope_factor;
   /* RoPE frequency scaling: 0 = linear (inv_freq / rope_factor; DeepSeek-Coder decoders of the v1 checkpoints),
