@@ -94,6 +94,17 @@ DTK_DEV void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t ba
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// the same copy with an L2 cache policy (createpolicy) attached
+DTK_DEV void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n" ::"r"(dst),
+               "l"(src), "r"(bytes), "r"(bar), "l"(pol)
+               : "memory");
+}
+DTK_DEV uint64_t policy_evict_first() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(pol));
+  return pol;
+}
 DTK_DEV void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMER_THREADS) : "memory"); }
 
 // ------------------------------------------------------------------ tagged activation words
@@ -392,6 +403,12 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
     asm volatile("setmaxnreg.dec.sync.aligned.u32 56;\n");
     const uint32_t pw = (uint32_t)(warp - NCW);
     if (lane == 0) {
+      // Weight tiles are read once per token and the stream (2.5 GB for ds-1.3b) is ~50x the L2: their lines are marked
+      // evict_first, so the L2 drops them before lines that are read again within the token (the tagged activation words
+      // every CTA polls). 3-4 % faster decode on the H100 (DESIGN.md section 9); the same policy on the key/value items was
+      // slower. (mega_variant bit 0: plain copies, for A/B runs.)
+      const bool evf = !(p.variant & 1);
+      const uint64_t pol = policy_evict_first();
       Walk w;
       uint32_t sl = pw, use = 0;   // ring slot / use count of this lane's next tile: its tiles are n = pw, pw + NPW, ... across ALL phases
       long long* tr = nullptr;   // dev trace: row (local tile index within the traced layer), column 0 = issue clock
@@ -431,7 +448,8 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
               bulk_g2s(dst + KV_V_OFF, kb + p.kv_v_offset, bytes, fb);
             } else {
               mbar_expect_tx(fb, TILE_BYTES);
-              bulk_g2s(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb);
+              if (evf) bulk_g2s_hint(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb, pol);
+              else bulk_g2s(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb);
             }
             if (DBG && tr) {
               const uint32_t row = w.nb + j - tr_nb0;

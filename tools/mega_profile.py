@@ -26,9 +26,9 @@ def timeit(label):
 import subprocess
 print(subprocess.run(["nvidia-smi", "--query-gpu=name,clocks.sm,clocks.mem,power.draw,temperature.gpu,clocks_event_reasons.active", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip())
 timeit("default")
-for variant in (1, 2, 3, 0, 2, 0):
+for variant in (1, 0, 1, 0):
     eng.set_option("mega_variant", variant)
-    timeit(f"variant={variant} (bit 0: coherent loads first when staging, bit 1: arrival counter before staging)")
+    timeit(f"variant={variant} (bit 0: weight copies without the evict_first L2 policy)")
     lgv = eng.decode([slot], [ctx], tok)[0].clone()
     if variant == 1:
         lg_ref = lgv
@@ -83,7 +83,7 @@ MHZ = 1965.0
 ntile = [24, 8, 40, 22] if "1.3b" in name else None
 print(f"\nper-tile trace of layer {TL} (us, SM clock at {MHZ:.0f} MHz, relative to the CTA's own layer start stamp)")
 print("columns per tile: issue(producer) landed asked done | landed-issue")
-for cta in (0, 1, 50, 100, 147):
+for cta in (0, 1, G // 3, 2 * G // 3, G - 1):
     d = tr[cta]
     t0c = d[160, 0]
     ph = (d[160:165] - t0c) / MHZ
