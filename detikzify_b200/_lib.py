@@ -72,6 +72,7 @@ SYMBOLS = {
     "dtk_seq_fork": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
     "dtk_seq_share": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
     "dtk_prefill": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "dtk_score": (C.c_int, [_P, C.c_int, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "dtk_decode": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, C.c_int, _P, _P]),
     "dtk_sample": (C.c_int, [_P, _P, C.c_int, C.POINTER(DtkSampling), C.POINTER(C.c_int),
                              C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P, _P, _P]),
@@ -88,6 +89,7 @@ SYMBOLS = {
     "dtk_dbg_mega_trace": (C.c_int, [_P, C.POINTER(C.c_longlong), C.c_int]),
     "dtk_dbg_gemm_impl": (C.c_int, [C.c_int]),
     "dtk_dbg_gemm": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "dtk_dbg_lm_logprob": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
     "dtk_dbg_flash_attn": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_float, _P]),
     "dtk_dbg_attn_tc": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P]),

@@ -22,6 +22,14 @@ DTK_DEV float warp_max(float v) {
   return v;
 }
 
+// log-sum-exp state (max m, sum s of exp(v - m)) absorbs another one; an empty state is (-inf, 0)
+DTK_DEV void lse_combine(float& m, float& s, float om, float os) {
+  const float nm = fmaxf(m, om);
+  if (nm == -INFINITY) return;
+  s = s * __expf(m - nm) + os * __expf(om - nm);
+  m = nm;
+}
+
 DTK_DEV uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // 16-byte async copy global->shared; src_bytes in {0,16}: 0 zero-fills the destination.

@@ -203,6 +203,9 @@ struct dtk_engine {
   // prefill workspace (max_len rows)
   float *p_x = nullptr, *p_qkv = nullptr;
   bf16 *p_xn = nullptr, *p_q = nullptr, *p_att = nullptr, *p_h = nullptr;
+  // scoring workspace (dtk_score; allocated at the first call): lm_head log-softmax partials [max_len, ceil(V / 256)], targets' logits
+  float2* lse_part = nullptr;
+  float* lse_tgt = nullptr;
   // decode workspace (max_batch rows)
   float *d_x = nullptr, *d_q = nullptr, *d_att = nullptr, *d_h = nullptr, *d_logits = nullptr, *d_scratch = nullptr;
   float *d_part_o = nullptr, *d_part_ml = nullptr;
@@ -888,7 +891,7 @@ int dtk_destroy(dtk_engine* eng) {
   void* ptrs[] = {eng->v_pix_in, eng->v_tok_out, eng->v_pool_out, eng->v_vt, eng->kv, eng->rope_cs, eng->p_x, eng->p_qkv, eng->p_xn, eng->p_q, eng->p_att, eng->p_h, eng->d_x, eng->d_q,
                   eng->d_att, eng->d_h, eng->d_logits, eng->d_scratch, eng->d_part_o, eng->d_part_ml, eng->d_counters,
                   eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
-                  eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b};
+                  eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt};
   for (void* p : ptrs) if (p) cudaFree(p);
   dtk_adapter_detach(eng);
   if (eng->cap_stream) cudaStreamDestroy(eng->cap_stream);
@@ -1231,9 +1234,11 @@ int dtk_seq_share(dtk_engine* eng, int base, int dst, int len, void* stream) {
   return r;
 }
 
-int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos, const float* img_embeds,
-                int img_start, int n_img, float* last_logits, float* all_logits, void* stream) {
-  if (!eng) return DTK_ERR_INVALID;
+namespace {
+// embedding splice + every decoder layer over ids[0..T) at positions [start_pos, start_pos + T) of `slot` (KV appended);
+// leaves the residual stream in p_x. Shared by dtk_prefill and dtk_score.
+int decoder_stack(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos, const float* img_embeds, int img_start,
+                  int n_img, cudaStream_t s) {
   const dtk_config& c = eng->cfg;
   DTK_REQUIRE(ids && T > 0, "ids/T");
   DTK_REQUIRE(slot >= 0 && slot < c.max_seqs, "slot");
@@ -1241,7 +1246,6 @@ int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_
   DTK_REQUIRE(start_pos >= eng->share_len[slot], "start_pos lies inside the sequence's shared (read-only) prefix");
   DTK_REQUIRE(start_pos >= eng->shared_upto[slot], "start_pos lies inside a prefix other sequences share from this slot");
   DTK_CK(cudaSetDevice(eng->device));
-  cudaStream_t s = (cudaStream_t)stream;
   uint64_t* lc = &eng->launches;
   const int H = c.hidden, I = c.inter, HD = c.head_dim, qd = c.heads * HD, kd = c.kv_heads * HD;
   DTK_CK(launch_embed_splice(ids, T, start_pos, W(eng, "dec.embed"), H, c.vocab, c.image_token_id, img_embeds, img_start,
@@ -1293,6 +1297,19 @@ int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_
       DTK_CK(launch_gemm(g, s, lc));
     }
   }
+  return DTK_OK;
+}
+}  // namespace
+
+int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos, const float* img_embeds,
+                int img_start, int n_img, float* last_logits, float* all_logits, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  const dtk_config& c = eng->cfg;
+  cudaStream_t s = (cudaStream_t)stream;
+  uint64_t* lc = &eng->launches;
+  const int H = c.hidden;
+  int r = decoder_stack(eng, slot, ids, T, start_pos, img_embeds, img_start, n_img, s);
+  if (r != DTK_OK) return r;
   if (last_logits) {  // final RMSNorm + lm_head on the last row only (reference computes all T rows, v1/modeling:251-257)
     GemvArgs g{};
     g.mode = GEMV_STORE; g.W = W(eng, "dec.lm_head"); g.N = c.vocab; g.K = H;
@@ -1307,6 +1324,29 @@ int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_
     g.out_f32 = all_logits; g.ldo = c.vocab;
     DTK_CK(launch_gemm(g, s, lc));
   }
+  return DTK_OK;
+}
+
+int dtk_score(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos, const float* img_embeds, int img_start,
+              int n_img, const int64_t* targets, float* logprob, float* lse, float* all_logits, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(targets && logprob, "targets/logprob");
+  cudaStream_t s = (cudaStream_t)stream;
+  uint64_t* lc = &eng->launches;
+  const int H = c.hidden;
+  int r = decoder_stack(eng, slot, ids, T, start_pos, img_embeds, img_start, n_img, s);
+  if (r != DTK_OK) return r;
+  // first scoring call: partials workspace for max_len rows (engines that never score do not pay it)
+  if (!eng->lse_part) DTK_ALLOC(eng->lse_part, (int64_t)c.max_len * ((c.vocab + LSE_TILE - 1) / LSE_TILE));
+  if (!eng->lse_tgt) DTK_ALLOC(eng->lse_tgt, c.max_len);
+  DTK_CK(launch_rmsnorm(eng->p_x, H, W(eng, "dec.norm"), c.rms_eps, T, H, eng->p_xn, s, lc));
+  GemmLseArgs g{};
+  g.A = eng->p_xn; g.lda = H; g.W = W(eng, "dec.lm_head"); g.ldw = H; g.M = T; g.N = c.vocab; g.K = H;
+  g.out_f32 = all_logits; g.ldo = c.vocab;
+  g.targets = targets; g.part = eng->lse_part; g.tgt = eng->lse_tgt;
+  DTK_CK(launch_gemm_lse(g, s, lc));
+  DTK_CK(launch_lse_merge(eng->lse_part, eng->lse_tgt, targets, T, c.vocab, logprob, lse, s, lc));
   return DTK_OK;
 }
 
@@ -1619,6 +1659,33 @@ int dtk_dbg_gemm(const void* A, const void* Wm, const void* bias, const float* r
   g.bias = (const bf16*)bias; g.resid = resid; g.ldr = glu ? N / 2 : N; g.act = act; g.glu = glu;
   g.out_f32 = out_f32; g.out_bf16 = (bf16*)out_bf16; g.ldo = glu ? N / 2 : N;
   return launch_gemm(g, (cudaStream_t)stream, nullptr) == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
+}
+
+int dtk_dbg_lm_logprob(const void* A, const void* Wm, int M, int N, int K, const int64_t* targets, float* logprob, float* lse,
+                       void* stream) {
+  if (!A || !Wm || !targets || !logprob || M <= 0 || N <= 0 || K <= 0) return DTK_ERR_INVALID;
+  // grow-only partials workspace of this test hook (per device; calls must not overlap)
+  static float2* part[64] = {};
+  static float* tgt[64] = {};
+  static int64_t cap_rows[64] = {}, cap_part[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return DTK_ERR_CUDA;
+  const int64_t np = (int64_t)M * ((N + LSE_TILE - 1) / LSE_TILE);
+  if (np > cap_part[dev] || M > cap_rows[dev]) {
+    cudaDeviceSynchronize();
+    cudaFree(part[dev]);
+    cudaFree(tgt[dev]);
+    part[dev] = nullptr; tgt[dev] = nullptr; cap_part[dev] = cap_rows[dev] = 0;
+    if (cudaMalloc(&part[dev], np * sizeof(float2)) != cudaSuccess || cudaMalloc(&tgt[dev], (size_t)M * sizeof(float)) != cudaSuccess)
+      return DTK_ERR_OOM;
+    cap_part[dev] = np; cap_rows[dev] = M;
+  }
+  GemmLseArgs g{};
+  g.A = (const bf16*)A; g.lda = K; g.W = (const bf16*)Wm; g.ldw = K; g.M = M; g.N = N; g.K = K;
+  g.targets = targets; g.part = part[dev]; g.tgt = tgt[dev];
+  if (launch_gemm_lse(g, (cudaStream_t)stream, nullptr) != cudaSuccess) return DTK_ERR_CUDA;
+  return launch_lse_merge(part[dev], tgt[dev], targets, M, N, logprob, lse, (cudaStream_t)stream, nullptr) == cudaSuccess
+             ? DTK_OK : DTK_ERR_CUDA;
 }
 
 int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void* o, int B, int heads, int Tq, int Tk,

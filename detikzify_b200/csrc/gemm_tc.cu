@@ -75,10 +75,57 @@ DTK_DEV void dense_store(const GemmArgs& p, int m, int n, float v0, float v1) {
   else *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(v0, v1);
 }
 
-// CTAs walk the output tiles (m fastest: concurrent CTAs share a BN-row band of W) with stride gridDim.x.
+// log-softmax epilogue of the lm_head (LSE instantiation, BN = 256): this thread holds rows r0 (i = 0) and r0 + 8 (i = 1)
+// at columns n0 + 8 j + 2 c + {0, 1}. Per row: {max, sum exp} over the valid columns (n < N; the TMA zero fill past V
+// stays out), reduced in the thread, then over the quad's 4 lanes by shuffle; lane c = 0 writes the tile's partial.
 template <int BN>
+DTK_DEV void lse_epilogue(const GemmLseArgs& p, const float (&acc)[BN / 2], int r0, int n0, int c) {
+  const int NT = (p.N + BN - 1) / BN, tj = n0 / BN;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int m = r0 + 8 * i;
+    float mx = -INFINITY, sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      if (n0 + 8 * j + 2 * c < p.N) mx = fmaxf(mx, fmaxf(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]));
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      if (n0 + 8 * j + 2 * c < p.N) sum += __expf(acc[4 * j + 2 * i] - mx) + __expf(acc[4 * j + 2 * i + 1] - mx);
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, mx, o), os = __shfl_xor_sync(0xffffffffu, sum, o);
+      lse_combine(mx, sum, om, os);
+    }
+    if (m >= p.M) continue;
+    if (c == 0) p.part[(int64_t)m * NT + tj] = make_float2(mx, sum);
+    const int64_t t = p.targets[m] - n0;
+    if (t >= 0 && t < BN && n0 + t < p.N && ((t & 7) >> 1) == c) {   // the target column is one of this thread's
+      const int jt = (int)(t >> 3);
+      float v = 0.f;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+        if (j == jt) v = (t & 1) ? acc[4 * j + 2 * i + 1] : acc[4 * j + 2 * i];
+      p.tgt[m] = v;
+    }
+    if (p.out_f32) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * c;
+        if (n < p.N) *reinterpret_cast<float2*>(p.out_f32 + (int64_t)m * p.ldo + n) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      }
+    }
+  }
+}
+
+template <bool LSE> struct DenseArgs { using type = GemmArgs; };
+template <> struct DenseArgs<true> { using type = GemmLseArgs; };
+
+// CTAs walk the output tiles (m fastest: concurrent CTAs share a BN-row band of W) with stride gridDim.x.
+// LSE = true: the lm_head's log-softmax epilogue instead of the generic one.
+template <int BN, bool LSE = false>
 __global__ void __launch_bounds__(DTHREADS, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA,
-                                                              const __grid_constant__ CUtensorMap mapB, const GemmArgs p) {
+                                                              const __grid_constant__ CUtensorMap mapB,
+                                                              const typename DenseArgs<LSE>::type p) {
   constexpr int STAGE_BYTES = DenseCfg<BN>::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;      // SWIZZLE_128B tiles need 1024-byte alignment
@@ -140,12 +187,16 @@ __global__ void __launch_bounds__(DTHREADS, 1) gemm_tc_kernel(const __grid_const
     if (lane == 0) mbar_arrive(empty0 + 8 * ((it - 1) % DSTAGES));
 
     const int r0 = m0 + wg * 64 + (warp & 3) * 16 + g;
+    if constexpr (LSE) {
+      lse_epilogue<BN>(p, acc, r0, n0, c);
+    } else {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = n0 + 8 * j + 2 * c;
-      if (n >= p.N) break;   // N is even: the pair (n, n + 1) is inside or outside together
-      if (r0 < p.M) dense_store(p, r0, n, acc[4 * j], acc[4 * j + 1]);
-      if (r0 + 8 < p.M) dense_store(p, r0 + 8, n, acc[4 * j + 2], acc[4 * j + 3]);
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * c;
+        if (n >= p.N) break;   // N is even: the pair (n, n + 1) is inside or outside together
+        if (r0 < p.M) dense_store(p, r0, n, acc[4 * j], acc[4 * j + 1]);
+        if (r0 + 8 < p.M) dense_store(p, r0 + 8, n, acc[4 * j + 2], acc[4 * j + 3]);
+      }
     }
   }
 }
@@ -329,8 +380,8 @@ bool gemm_tc_supported(const GemmArgs& a) {
 }
 
 // persistent = one CTA per SM walks the tiles; otherwise one CTA per tile
-template <int BN>
-static cudaError_t launch_tc_dense(const GemmArgs& a, bool persistent, cudaStream_t s, uint64_t* counter) {
+template <int BN, bool LSE = false>
+static cudaError_t launch_tc_dense(const typename DenseArgs<LSE>::type& a, bool persistent, cudaStream_t s, uint64_t* counter) {
   CUtensorMap mapA, mapB;
   if (!make_map(&mapA, a.A, a.M, a.K, a.lda, TBM) || !make_map(&mapB, a.W, a.N, a.K, a.ldw, BN)) return cudaErrorInvalidValue;
   constexpr int smem = DenseCfg<BN>::SMEM;
@@ -342,14 +393,14 @@ static cudaError_t launch_tc_dense(const GemmArgs& a, bool persistent, cudaStrea
   if (e != cudaSuccess) return e;
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (!attr_done[dev]) {
-    e = cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    e = cudaFuncSetAttribute(gemm_tc_kernel<BN, LSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
     e = cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return e;
     attr_done[dev] = true;
   }
   const int tiles = ((a.M + TBM - 1) / TBM) * ((a.N + BN - 1) / BN);
-  gemm_tc_kernel<BN><<<persistent && tiles > sms[dev] ? sms[dev] : tiles, DTHREADS, smem, s>>>(mapA, mapB, a);
+  gemm_tc_kernel<BN, LSE><<<persistent && tiles > sms[dev] ? sms[dev] : tiles, DTHREADS, smem, s>>>(mapA, mapB, a);
   if (counter) ++*counter;
   return cudaGetLastError();
 }
@@ -408,6 +459,15 @@ cudaError_t launch_gemm_tc(const GemmArgs& a, cudaStream_t s, uint64_t* counter)
   // no such epilogue, so these few small products run on a 128-row tile that is mostly TMA zero fill
   if (get_gemm_impl() == 2) return launch_tc_dense<256>(a, true, s, counter);   // persistent 128 x 256
   return launch_tc_dense<128>(a, false, s, counter);
+}
+
+cudaError_t launch_gemm_lse(const GemmLseArgs& a, cudaStream_t s, uint64_t* counter) {
+  if (a.M <= 0 || a.N <= 0 || a.K <= 0) return cudaSuccess;
+  if (!a.targets || !a.part || !a.tgt || a.bias || a.rowbias || a.resid || a.act != ACT_NONE || a.glu || a.gate || a.out_bf16 ||
+      (a.out_f32 && a.ldo != a.N) || !gemm_tc_supported(a))
+    return cudaErrorInvalidValue;
+  // every M runs on the dense tile (a small M is mostly TMA zero fill): the swapped and mma.sync tiles have no such epilogue
+  return launch_tc_dense<LSE_TILE, true>(a, true, s, counter);
 }
 
 }  // namespace dtk

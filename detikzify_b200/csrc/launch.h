@@ -38,6 +38,21 @@ cudaError_t launch_gemm(const GemmArgs& a, cudaStream_t s, uint64_t* counter);  
 cudaError_t launch_gemm_mma(const GemmArgs& a, cudaStream_t s, uint64_t* counter);
 cudaError_t launch_gemm_tc(const GemmArgs& a, cudaStream_t s, uint64_t* counter);
 bool gemm_tc_supported(const GemmArgs& a);
+// lm_head GEMM with a log-softmax epilogue (persistent 128 x 256 wgmma kernel, every M): for each row m < M and 256-column
+// tile j of C = A W^T, part[m * ceil(N / 256) + j] = {max, sum exp(v - max)} over the tile's columns n < N, and
+// tgt[m] = C[m, targets[m]] when targets[m] is in [0, N). C itself is stored only when out_f32 is non-null (ldo = N); the
+// other epilogue fields of GemmArgs must be off. Deterministic: no atomics, fixed reduction order.
+struct GemmLseArgs : GemmArgs {
+  const int64_t* targets;     // [M] (any value; outside [0, N) = no target)
+  float2* part;               // [M, ceil(N / 256)]
+  float* tgt;                 // [M]
+};
+constexpr int LSE_TILE = 256;
+cudaError_t launch_gemm_lse(const GemmLseArgs& a, cudaStream_t s, uint64_t* counter);
+// folds the partials of each row in a fixed order: lse[m] (may be null) = log sum exp C[m, :N],
+// logprob[m] = tgt[m] - lse[m] when targets[m] is in [0, N), else 0
+cudaError_t launch_lse_merge(const float2* part, const float* tgt, const int64_t* targets, int M, int N, float* logprob,
+                             float* lse, cudaStream_t s, uint64_t* counter);
 void set_gemm_swap_split(int v);    // dev: 0 (default) = heuristic split-K factor of the swapped tile, 1..8 = forced
 void set_gemm_impl(int impl);   // 0 = mma.sync everywhere, 1 = wgmma one 128 x 128 tile per CTA, 2 = persistent 128 x 256 wgmma (process-wide dev switch)
 int get_gemm_impl();

@@ -370,8 +370,40 @@ __global__ void __launch_bounds__(128) pool_attn_kernel(const float* __restrict_
   }
 }
 
+// lm_head log-softmax merge: one warp per row; lane l folds the tile partials l, l + 32, ... in order, then a fixed
+// xor tree combines the lanes (deterministic)
+__global__ void __launch_bounds__(256) lse_merge_kernel(const float2* __restrict__ part, const float* __restrict__ tgt,
+                                                        const int64_t* __restrict__ targets, int M, int N, int NT,
+                                                        float* __restrict__ logprob, float* __restrict__ lse) {
+  const int m = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (m >= M) return;
+  float mx = -INFINITY, s = 0.f;
+  for (int j = lane; j < NT; j += 32) {
+    const float2 q = part[(int64_t)m * NT + j];
+    lse_combine(mx, s, q.x, q.y);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+    lse_combine(mx, s, om, os);
+  }
+  if (lane == 0) {
+    const float l = mx + logf(s);
+    const int64_t t = targets[m];
+    logprob[m] = (t >= 0 && t < N) ? tgt[m] - l : 0.f;
+    if (lse) lse[m] = l;
+  }
+}
+
 }  // namespace
 
+cudaError_t launch_lse_merge(const float2* part, const float* tgt, const int64_t* targets, int M, int N, float* logprob,
+                             float* lse, cudaStream_t s, uint64_t* counter) {
+  if (M <= 0) return cudaSuccess;
+  lse_merge_kernel<<<(M + 7) / 8, 256, 0, s>>>(part, tgt, targets, M, N, (N + LSE_TILE - 1) / LSE_TILE, logprob, lse);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
 cudaError_t launch_layernorm(const float* x, const bf16* w, const bf16* b, float eps, int M, int D, bf16* out_bf16,
                              float* out_f32, cudaStream_t s, uint64_t* counter) {
   if (D & 3) return cudaErrorInvalidValue;

@@ -365,6 +365,36 @@ class Engine:
                                          n_img, self._ptr(last), self._ptr(alll), self._stream()), "dtk_prefill")
         return last, alll
 
+    def score(self, slot: int, ids: torch.Tensor, start_pos: int = 0, img_embeds: Optional[torch.Tensor] = None,
+              img_start: int = 0, targets: Optional[torch.Tensor] = None, want_all_logits: bool = False, *,
+              logits_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+        """Prefill ids int64 [T] like ``prefill`` and score every row with the fused lm_head log-softmax. ``targets`` int64 [T]
+        (negative = none). Returns (logprob fp32 [T] (0 where there is no target), lse fp32 [T], all_logits fp32 [T,V] | None).
+        ``logits_out``: a contiguous fp32 [T,V] device tensor (e.g. rows of a larger batch output) that receives the logits."""
+        if targets is None:
+            raise ValueError("score() needs targets: int64 [T], negative = no target")
+        ids = ids.to(self.device, torch.int64).contiguous().view(-1)
+        T = ids.numel()
+        targets = targets.to(self.device, torch.int64).contiguous().view(-1)
+        if targets.numel() != T:
+            raise ValueError(f"targets must hold one entry per id ({targets.numel()} != {T})")
+        if logits_out is not None:
+            if logits_out.device != self.device or logits_out.dtype != torch.float32 or not logits_out.is_contiguous() \
+                    or logits_out.numel() != T * self.Vocab:
+                raise ValueError("logits_out must be a contiguous fp32 [T, V] tensor on the engine's device")
+        elif want_all_logits:
+            logits_out = torch.empty(T, self.Vocab, device=self.device, dtype=torch.float32)
+        logprob = torch.empty(T, device=self.device, dtype=torch.float32)
+        lse = torch.empty(T, device=self.device, dtype=torch.float32)
+        n_img = 0
+        if img_embeds is not None:
+            img_embeds = img_embeds.to(self.device, torch.float32).contiguous().view(-1, self.H)
+            n_img = img_embeds.shape[0]
+        self._check(self.lib.dtk_score(self._h, slot, self._ptr(ids), T, start_pos, self._ptr(img_embeds), img_start, n_img,
+                                       self._ptr(targets), self._ptr(logprob), self._ptr(lse), self._ptr(logits_out),
+                                       self._stream()), "dtk_score")
+        return logprob, lse, logits_out
+
     def decode(self, slots: Sequence[int], positions: Sequence[int], ids: torch.Tensor) -> torch.Tensor:
         B = len(slots)
         ids = ids.to(self.device, torch.int64).contiguous().view(-1)

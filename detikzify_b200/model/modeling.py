@@ -22,7 +22,7 @@ from __future__ import annotations
 import threading
 from contextlib import nullcontext
 from types import SimpleNamespace
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -41,6 +41,26 @@ class GenerationConfig:
 
 class VisionOutput(SimpleNamespace):
     pass
+
+
+class CausalLMOutput:
+    """``forward()`` result: ``.loss`` (fp32 scalar or None), ``.logits`` (fp32 [B,T,V]), ``.past_key_values`` (always None).
+    Like HF's ModelOutput it also indexes by key (``out["logits"]``) and by position over the set fields (``out[0]``)."""
+
+    def __init__(self, loss: Optional[torch.Tensor], logits: torch.Tensor):
+        self.loss, self.logits, self.past_key_values = loss, logits, None
+
+    def to_tuple(self) -> tuple:
+        return tuple(v for v in (self.loss, self.logits) if v is not None)
+
+    def __getitem__(self, key):
+        return getattr(self, key) if isinstance(key, str) else self.to_tuple()[key]
+
+    def __iter__(self):
+        return iter(self.to_tuple())
+
+    def __len__(self) -> int:
+        return len(self.to_tuple())
 
 
 class DetikzifyVisionModel:
@@ -254,6 +274,77 @@ class DetikzifyForCausalLM:
         except (TypeError, IndexError):
             return default
 
+    # ---- prompt helpers shared by generate_batch / forward / score ----------------------------------
+    def _image_span(self, ids_host: List[int]) -> Tuple[int, int]:
+        """(start, count) of the image-token span of a prompt, (0, 0) without one; splice validation as
+        v1/modeling_detikzify.py:176-184."""
+        patch = self.config.image_token_id
+        n = ids_host.count(patch)
+        if n == 0:
+            return 0, 0
+        if n != self.config.num_patches:
+            raise ValueError("The number of image patch tokens should be the same as the number of image patches.")
+        st = ids_host.index(patch)
+        if ids_host[st: st + n] != [patch] * n:
+            raise ValueError("The image patch tokens should be consecutive.")
+        return st, n
+
+    @staticmethod
+    def _shared_prefix(prompts: Sequence[List[int]], lim: int, span: Tuple[int, int]) -> int:
+        """Longest common token prefix of the prompts, at most ``lim`` long; never splits the image span ``span`` of prompt 0
+        and is 0 below 16 positions (a shorter shared prefix saves less than the sharing costs)."""
+        lcp = 0
+        while lcp < lim and all(p[lcp] == prompts[0][lcp] for p in prompts[1:]):
+            lcp += 1
+        st0, n0 = span
+        if n0 and st0 < lcp < st0 + n0:
+            lcp = st0
+        return lcp if lcp >= 16 else 0
+
+    def _batch_captions(self, adapter_input_ids, adapter_attention_mask, pixel_values, N: int):
+        """TikZero captions of an N-sequence call (one shared or one per sequence) and the pixels to condition: a caption
+        without an image runs on the adapter's dummy image."""
+        captions = None
+        if adapter_input_ids is not None:
+            captions = self._captions(adapter_input_ids, adapter_attention_mask)
+            if len(captions) not in (1, N):
+                raise ValueError("adapter_input_ids must hold one caption (shared) or one caption per sequence")
+            if pixel_values is None:
+                pixel_values = self.adapter.dummy_pixels()
+        return captions, pixel_values
+
+    def _batch_image_embeds(self, pixel_values: Optional[torch.Tensor], captions, N: int) -> Optional[torch.Tensor]:
+        """Image embeddings [1 | N, P, H] for one shared image or one image per sequence (None without pixels)."""
+        if pixel_values is None:
+            return None
+        eng = self.engine
+        pix = pixel_values.to(self.device, torch.float32)
+        if pix.dim() == 3:
+            pix = pix[None]
+        if pix.shape[0] not in (1, N):
+            raise ValueError("pixel_values must hold one image (shared) or one image per sequence")
+        if captions is None:
+            return eng.image_embeds(pix)
+        # one conditioned tower pass per distinct (image, caption) pairing
+        if pix.shape[0] != len(captions):
+            pix = pix.expand(N, *pix.shape[1:]).contiguous()
+            captions = captions * N if len(captions) == 1 else captions
+        return eng.image_embeds_cond(pix, [torch.tensor(c) for c in captions])
+
+    def _to_device_ids(self, ids_host: List[int]) -> torch.Tensor:
+        t = torch.tensor(ids_host, dtype=torch.int64)
+        return t.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else t
+
+    def _scratch_slot(self) -> Tuple[int, bool]:
+        """An engine slot for a call that keeps no KV state: a free one (owned: the caller frees it) or, when none is free,
+        the least recently used prefix-cache slot of generate(), whose cached content is forgotten (not owned)."""
+        try:
+            return self.engine.seq_alloc(), True
+        except Exception:
+            kv = min(self._kv, key=lambda k: k.tick)
+            kv.tokens = []
+            return kv.slot, False
+
     # ---- generate --------------------------------------------------------------------------------
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor = None, pixel_values: Optional[torch.Tensor] = None,
@@ -402,13 +493,7 @@ class DetikzifyForCausalLM:
         N = len(prompts)
         if N == 0:
             return []
-        captions = None
-        if adapter_input_ids is not None:
-            captions = self._captions(adapter_input_ids, adapter_attention_mask)
-            if len(captions) not in (1, N):
-                raise ValueError("adapter_input_ids must hold one caption (shared) or one caption per sequence")
-            if pixel_values is None:
-                pixel_values = self.adapter.dummy_pixels()
+        captions, pixel_values = self._batch_captions(adapter_input_ids, adapter_attention_mask, pixel_values, N)
         if any(len(p) == 0 for p in prompts):
             raise ValueError("empty prompt")
         streamers = list(streamers) if streamers is not None else [None] * N
@@ -424,34 +509,8 @@ class DetikzifyForCausalLM:
         for p in prompts:
             ml = max_length if max_length is not None else (len(p) + max_new_tokens if max_new_tokens is not None else gc.max_length)
             limits.append(min(int(ml), eng.max_len))
-        patch = cfg.image_token_id
-
-        def spans(ids_host):
-            n = ids_host.count(patch)
-            if n == 0:
-                return 0, 0
-            if n != cfg.num_patches:   # splice validation (v1/modeling_detikzify.py:176-184)
-                raise ValueError("The number of image patch tokens should be the same as the number of image patches.")
-            st = ids_host.index(patch)
-            if ids_host[st: st + n] != [patch] * n:
-                raise ValueError("The image patch tokens should be consecutive.")
-            return st, n
-
         with self._lock, self._on_stream():
-            imgs = None
-            if pixel_values is not None:
-                pix = pixel_values.to(self.device, torch.float32)
-                if pix.dim() == 3:
-                    pix = pix[None]
-                if pix.shape[0] not in (1, N):
-                    raise ValueError("pixel_values must hold one image (shared) or one image per sequence")
-                if captions is None:
-                    imgs = eng.image_embeds(pix)
-                else:   # one conditioned tower pass per distinct (image, caption) pairing
-                    if pix.shape[0] != len(captions):
-                        pix = pix.expand(N, *pix.shape[1:]).contiguous()
-                        captions = captions * N if len(captions) == 1 else captions
-                    imgs = eng.image_embeds_cond(pix, [torch.tensor(c) for c in captions])
+            imgs = self._batch_image_embeds(pixel_values, captions, N)
             for i, st in enumerate(streamers):
                 if st is not None:
                     st.put(torch.tensor([prompts[i]], dtype=torch.int64))
@@ -464,38 +523,27 @@ class DetikzifyForCausalLM:
                 lcp = 0
                 one_image = imgs is None or imgs.shape[0] == 1
                 if share_prefix and N > 1 and one_image:
-                    lim = min(len(p) for p in prompts) - 1
-                    while lcp < lim and all(p[lcp] == prompts[0][lcp] for p in prompts[1:]):
-                        lcp += 1
-                    st0, n0 = spans(prompts[0][:]) if imgs is not None else (0, 0)
-                    if n0 and st0 < lcp < st0 + n0:
-                        lcp = st0
-                    if lcp < 16:
-                        lcp = 0
+                    lcp = self._shared_prefix(prompts, min(len(p) for p in prompts) - 1,
+                                              self._image_span(prompts[0]) if imgs is not None else (0, 0))
                 if lcp:
                     try:
                         base_slot = eng.seq_alloc()
                     except Exception:       # no spare slot: every sequence prefills its whole prompt
                         base_slot, lcp = None, 0
                 if lcp:
-                    st0, n0 = spans(prompts[0]) if imgs is not None else (0, 0)
-                    head = torch.tensor(prompts[0][:lcp], dtype=torch.int64)
-                    if self.device.type == "cuda":
-                        head = head.pin_memory().to(self.device, non_blocking=True)
+                    st0, n0 = self._image_span(prompts[0]) if imgs is not None else (0, 0)
+                    head = self._to_device_ids(prompts[0][:lcp])
                     eng.prefill(base_slot, head, 0, imgs[0] if (imgs is not None and n0 and st0 < lcp) else None, st0)
                 last = []
                 for i, ids_host in enumerate(prompts):
                     img, img_start = None, 0
                     if imgs is not None:
-                        img_start, n_patch = spans(ids_host)
+                        img_start, n_patch = self._image_span(ids_host)
                         if n_patch and img_start >= lcp:
                             img = imgs[i if imgs.shape[0] == N else 0]
                     if lcp:
                         eng.seq_share(base_slot, slots[i], lcp)
-                    ids_dev = torch.tensor(ids_host[lcp:], dtype=torch.int64)
-                    if self.device.type == "cuda":
-                        ids_dev = ids_dev.pin_memory().to(self.device, non_blocking=True)
-                    lg, _ = eng.prefill(slots[i], ids_dev, lcp, img, img_start)
+                    lg, _ = eng.prefill(slots[i], self._to_device_ids(ids_host[lcp:]), lcp, img, img_start)
                     last.append(lg)
                 self._call_counter += 1
                 params = eng.sampling(
@@ -545,6 +593,158 @@ class DetikzifyForCausalLM:
                     eng.seq_free(s)
                 if base_slot is not None:
                     eng.seq_free(base_slot)
+
+    # ---- logits, loss and sequence scoring ---------------------------------------------------------
+    def __call__(self, *args, **kwargs):
+        return self.forward(*args, **kwargs)
+
+    @torch.no_grad()
+    def forward(self, input_ids: torch.Tensor = None, pixel_values: Optional[torch.Tensor] = None,
+                attention_mask: Optional[torch.Tensor] = None, labels: Optional[torch.Tensor] = None,
+                adapter_input_ids=None, adapter_attention_mask=None, logits_to_keep=None, return_dict: Optional[bool] = None,
+                **ignored) -> Union[CausalLMOutput, tuple]:
+        """The reference's ``forward`` (v1/modeling_detikzify.py:218-283, modeling_detikzify.py:320-389): fp32 logits
+        [B,T,V] for every position and, with ``labels``, the mean cross-entropy of the shifted labels (``-100`` ignored; v2
+        checkpoints with an ``attention_mask`` count only shifted positions whose mask is set). No gradients, no KV state.
+
+        Each row runs unpadded through one engine call that writes its logits into the output and the log-probs of its
+        shifted labels (fused lm_head log-softmax, no cross-entropy over the logits). ``attention_mask`` must be one
+        contiguous run of ones per row (left or right padding); logits at masked positions are 0, where HF returns
+        whatever the padded rows compute. RoPE sees only relative positions, so the logits match HF's up to rounding.
+        ``logits_to_keep`` is accepted and ignored, as the reference does; ``use_cache`` is ignored."""
+        for key in ("inputs_embeds", "past_key_values"):
+            if ignored.get(key) is not None:
+                raise ValueError(f"forward() does not take `{key}`: it runs whole sequences from input_ids and keeps no KV cache")
+        for key in ("output_attentions", "output_hidden_states"):
+            if ignored.get(key):
+                raise ValueError(f"forward() does not return {key[len('output_'):]}")
+        cfg, eng, V = self.config, self.engine, self.config.vocab_size
+        ids = torch.as_tensor(input_ids).cpu()
+        ids = ids[None] if ids.dim() == 1 else ids
+        B, T = ids.shape
+        if T == 0:
+            raise ValueError("empty input_ids")
+        if T > eng.max_len:
+            raise ValueError(f"sequence length {T} exceeds the engine's max_len {eng.max_len}")
+        mask = None if attention_mask is None else torch.as_tensor(attention_mask).cpu().reshape(B, T) != 0
+        runs = []
+        for b in range(B):
+            if mask is None:
+                runs.append((0, T))
+                continue
+            on = mask[b].nonzero().view(-1)
+            if on.numel() == 0 or int(on[-1]) - int(on[0]) + 1 != on.numel():
+                raise ValueError("attention_mask must hold one contiguous run of ones per row (left or right padding)")
+            runs.append((int(on[0]), int(on[-1]) + 1))
+        # targets of row t: the label of position t + 1 where the reference's loss counts it, else -1
+        targets = torch.full((B, T), -1, dtype=torch.int64)
+        count = 0
+        if labels is not None:
+            sh = torch.as_tensor(labels).cpu().reshape(B, T)[:, 1:].to(torch.int64)
+            use = sh != -100
+            if not cfg.projector_bias and mask is not None:   # v2: attention_mask[:, 1:] != 0 selects the counted positions
+                use &= mask[:, 1:]
+            if mask is not None and (use & ~mask[:, :-1]).any():
+                raise ValueError("a counted label is predicted from a masked position (set it to -100)")
+            if (use & ((sh < 0) | (sh >= V))).any():
+                raise ValueError(f"labels must be -100 or in [0, {V})")
+            targets[:, :-1] = torch.where(use, sh, torch.full_like(sh, -1))
+            count = int(use.sum())
+        rows = [ids[b, a:e].tolist() for b, (a, e) in enumerate(runs)]
+        captions, pixel_values = self._batch_captions(adapter_input_ids, adapter_attention_mask, pixel_values, B)
+        spans = [self._image_span(r) if pixel_values is not None else (0, 0) for r in rows]
+
+        with self._lock, self._on_stream():
+            imgs = self._batch_image_embeds(pixel_values, captions, B) if any(n for _, n in spans) else None
+            logits = torch.zeros(B, T, V, device=self.device, dtype=torch.float32)
+            total = torch.zeros((), device=self.device, dtype=torch.float32)
+            slot, owned = self._scratch_slot()
+            try:
+                for b, (a, e) in enumerate(runs):
+                    st, n = spans[b]
+                    img = imgs[b if imgs.shape[0] == B else 0] if n else None
+                    lp, _, _ = eng.score(slot, self._to_device_ids(rows[b]), 0, img, st, targets[b, a:e].to(self.device),
+                                         logits_out=logits[b, a:e])
+                    if labels is not None:
+                        total += lp.sum()
+            finally:
+                if owned:
+                    eng.seq_free(slot)
+            loss = -total / count if labels is not None else None   # 0 / 0 = NaN when nothing is counted, as in torch
+            self._sync()
+        if return_dict is False:
+            return (loss, logits) if loss is not None else (logits,)
+        return CausalLMOutput(loss, logits)
+
+    @torch.no_grad()
+    def score(self, sequences: Sequence[torch.Tensor], pixel_values: Optional[torch.Tensor] = None, *,
+              start: Union[int, Sequence[int]] = 1, adapter_input_ids=None, adapter_attention_mask=None) -> List[torch.Tensor]:
+        """Log-likelihood of N id sequences (1-D) under the model, e.g. to rank candidate programs for one figure or to
+        measure perplexity. Returns one fp32 device tensor per sequence: entry k of sequence i is
+        log p(ids_i[start_i + k] | ids_i[:start_i + k]), for 1 <= start_i < len_i (``start``: one int or one per sequence).
+        ``pixel_values``: one shared image or one per sequence, as in ``generate_batch``; TikZero captions likewise.
+
+        The longest common prefix of the sequences (at most min(start_i) positions, never splitting an image span, none
+        below 16) is prefilled once into a base slot. Sequence i borrows its first s_i = min(lcp, start_i - 1) positions
+        from there and runs only ids_i[s_i : len_i - 1] through the fused lm_head log-softmax, so every scored row is
+        computed in its own prefill and no [T, V] logits are materialised. When a sequence's scoring starts right after the
+        shared prefix (start_i = lcp, e.g. a program right after the image span of a v1 prompt), it recomputes that one
+        last shared row. Uses two engine slots for any N.
+
+        Against ``forward()`` of each sequence alone the log-probs agree to about 1e-3 when a sequence's own prefill
+        has at least 64 rows. With fewer rows the decoder GEMMs run on the swapped-operand tile, whose bf16 activations
+        round differently, and the difference grows to about 1e-2 over 24 layers (random-init ds-1.3b weights)."""
+        seqs: List[List[int]] = [torch.as_tensor(q).reshape(-1).tolist() for q in sequences]
+        N = len(seqs)
+        if N == 0:
+            return []
+        starts = [int(start)] * N if isinstance(start, int) else [int(x) for x in start]
+        if len(starts) != N:
+            raise ValueError("start must be one int or one int per sequence")
+        for q, st in zip(seqs, starts):
+            if not 1 <= st < len(q):
+                raise ValueError(f"start must satisfy 1 <= start < len(sequence) (got {st} for length {len(q)})")
+            if len(q) > self.engine.max_len:
+                raise ValueError(f"sequence length {len(q)} exceeds the engine's max_len {self.engine.max_len}")
+        captions, pixel_values = self._batch_captions(adapter_input_ids, adapter_attention_mask, pixel_values, N)
+        eng = self.engine
+        with self._lock, self._on_stream():
+            imgs = self._batch_image_embeds(pixel_values, captions, N)
+            spans = [self._image_span(q) if imgs is not None else (0, 0) for q in seqs]
+            lcp = 0
+            if N > 1 and (imgs is None or imgs.shape[0] == 1):
+                lcp = self._shared_prefix(seqs, min(starts), spans[0])
+            work, owned = self._scratch_slot()
+            base = None
+            try:
+                if lcp:
+                    try:
+                        base = eng.seq_alloc()
+                    except Exception:       # no spare slot (the working slot was borrowed too): no sharing
+                        lcp = 0
+                if lcp:
+                    st0, n0 = spans[0]
+                    eng.prefill(base, self._to_device_ids(seqs[0][:lcp]), 0,
+                                imgs[0] if (imgs is not None and n0 and st0 < lcp) else None, st0)
+                out = []
+                for i, q in enumerate(seqs):
+                    s0 = min(lcp, starts[i] - 1)              # positions borrowed from the base slot
+                    st, n = spans[i]
+                    img = imgs[i if imgs.shape[0] == N else 0] if (imgs is not None and n and st + n > s0) else None
+                    if s0:
+                        eng.seq_share(base, work, s0)
+                    # row r sits at position s0 + r and predicts q[s0 + r + 1]; rows before start_i - 1 are not scored
+                    skip = starts[i] - 1 - s0
+                    tg = [-1] * skip + q[starts[i]:]
+                    lp, _, _ = eng.score(work, self._to_device_ids(q[s0:-1]), s0, img, st, self._to_device_ids(tg))
+                    out.append(lp[skip:])
+                self._sync()
+                return out
+            finally:
+                if owned:
+                    eng.seq_free(work)   # also ends its borrowing from the base slot
+                if base is not None:
+                    eng.seq_free(base)
 
     # ---- SelfSim helper: pooled features straight from the engine --------------------------------
     @torch.no_grad()

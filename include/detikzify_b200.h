@@ -180,6 +180,18 @@ DTK_API int dtk_prefill(dtk_engine* eng, int slot, const int64_t* ids, int T, in
                 const float* img_embeds, int img_start, int n_img,
                 float* last_logits, float* all_logits, void* stream);
 
+/* ---- sequence scoring. Replaces the logits + CrossEntropyLoss tail of DetikzifyForCausalLM.forward(labels=...)
+ *      (v1/modeling_detikzify.py:218-270, modeling_detikzify.py:320-376) without materialising [T,V] logits. Prefills
+ *      exactly as dtk_prefill (same preconditions, KV writes and shared-prefix rules), then applies the final RMSNorm to
+ *      all T rows and runs the lm_head GEMM with a fused log-softmax. targets: device int64 [T], a negative (or >= V)
+ *      value means "no target"; logprob: device fp32 [T] = log softmax(logits[t])[targets[t]] (0 without a target);
+ *      lse (may be NULL): device fp32 [T] = log sum exp logits[t]; all_logits (may be NULL): fp32 [T,V], the same values
+ *      the log-softmax was taken from. Deterministic. The first call allocates max_len * ceil(V/256) * 8 bytes of
+ *      workspace. ------------------------------------------------------------------------------------------------- */
+DTK_API int dtk_score(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos,
+                      const float* img_embeds, int img_start, int n_img, const int64_t* targets,
+                      float* logprob, float* lse, float* all_logits, void* stream);
+
 /* ---- single-token decode for B sequences (LlamaModel.forward with cache, q_len == 1;
  *      v1/modeling_detikzify.py:285-305). slots: host int[B]; positions host int[B] (the
  *      position the token occupies); ids: device int64[B]; logits: device fp32 [B,V]. ------ */
@@ -242,6 +254,11 @@ DTK_API int dtk_dbg_gemm_impl(int impl);
 DTK_API int dtk_dbg_gemm(const void* A_bf16, const void* W_bf16, const void* bias_bf16,
                          const float* resid, int M, int N, int K, int act, int glu,
                          float* out_f32, void* out_bf16, void* stream);
+/* lm_head log-softmax of dtk_score on its own: logprob[m] = log softmax(A W^T)[m, targets[m]] (0 when the target is outside
+ * [0, N)), lse (may be NULL) [M]; A bf16 [M,K], W bf16 [N,K], targets int64 [M]. Keeps a grow-only workspace per device:
+ * calls must not overlap. */
+DTK_API int dtk_dbg_lm_logprob(const void* A_bf16, const void* W_bf16, int M, int N, int K, const int64_t* targets,
+                               float* logprob, float* lse, void* stream);
 /* q,k,v,o bf16 [B, T, heads, head_dim]; head_dim in {72,128} */
 DTK_API int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void* o, int B,
                                int heads, int Tq, int Tk, int head_dim, int causal, int q_pos0,
