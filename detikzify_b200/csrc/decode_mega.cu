@@ -35,6 +35,8 @@
 // in the kernel tail). DESIGN.md section 4 describes the design.
 //
 // Replaces the per-token HF eager path (modeling_llama.py:303-333, ~900 launches per token).
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "launch.h"
 
@@ -106,6 +108,26 @@ DTK_DEV uint64_t policy_evict_first() {
   return pol;
 }
 DTK_DEV void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMER_THREADS) : "memory"); }
+
+// ------------------------------------------------------------------ e4m3 codes
+// two e4m3 codes (low 16 bits of v: low byte = first element) -> their values (exact in fp32)
+DTK_DEV float2 e4m3x2_to_float2(uint32_t v) {
+  uint32_t h;
+  asm("{\n\t.reg .b16 t;\n\tcvt.u16.u32 t, %1;\n\tcvt.rn.f16x2.e4m3x2 %0, t;\n\t}\n" : "=r"(h) : "r"(v));
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// the bf16 pair of an A fragment: two codes times the row scale 2^k_r (exact: the product is a bf16 value)
+DTK_DEV uint32_t e4m3x2_to_bf16x2(uint32_t v, float scale) {
+  const float2 f = e4m3x2_to_float2(v);
+  return pack_bf16x2(f.x * scale, f.y * scale);
+}
+// (a, b) -> two e4m3 codes (round to nearest even, saturating), a in the low byte
+DTK_DEV uint32_t float2_to_e4m3x2(float a, float b) {
+  uint16_t d;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;\n" : "=h"(d) : "f"(b), "f"(a));
+  return d;
+}
+DTK_DEV float pow2f(int k) { return __uint_as_float((uint32_t)(k + 127) << 23); }   // k in [-126, 127]
 
 // ------------------------------------------------------------------ tagged activation words
 // Every activation value that crosses CTAs (residual stream, q, the new key/value row, attention partials and output,
@@ -325,7 +347,9 @@ DTK_DEV float slices_rn(const float* slice_ss, int nslice, int K, float eps) {
 // then lm_head) with a single copy of the tile code and a run-time phase switch in the epilogue: the per-token
 // instruction footprint of a warp stays inside the SM's 32 KB instruction cache (the fully specialised version was
 // ~160 KB, re-fetched from L2 every layer: the first tiles of every phase ran 3-6x slower than the steady state).
-template <bool DBG, int HD>
+// F8 = true: the four layer matrices stream as e4m3 tiles (MegaF8); the consumers turn each A fragment into the bf16 bits
+// of code x 2^k_r and run the same mma sequence, so the logits equal those of the bf16 kernel on the dequantised weights.
+template <bool DBG, int HD, bool F8>
 __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const MegaArgs p) {
   constexpr int HALF = HD / 2;
   constexpr int LPK = HD / 8;                // attention: lanes per key (8 bf16 each)
@@ -435,6 +459,12 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
                                 : m.base + (int64_t)l * m.layer_stride + (int64_t)g0 * tpg * MEGA_TILE_ELEMS;
         // own tiles j = j0, j0 + NPW, ...
         uint32_t j = (pw + NPW - (w.nb & (NPW - 1))) & (NPW - 1);
+        MegaF8 f8{};
+        uint32_t jk = 0, jks = j;   // F8: tile j = group jk of the CTA's block, k-tile jks
+        if (F8) {
+          if (!attn && ph != PH_LM) f8 = p.f8[mat_of(ph)];
+          while (jks >= (uint32_t)tpg) { jks -= tpg; ++jk; }
+        }
         if ((int)j < ntiles) {
           for (; (int)j < ntiles; j += NPW) {
             if (use > 0) mbar_wait(empty0 + 8 * sl, (use - 1) & 1);
@@ -446,6 +476,13 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
               mbar_expect_tx(fb, 2 * bytes);
               bulk_g2s(dst, kb, bytes, fb);
               bulk_g2s(dst + KV_V_OFF, kb + p.kv_v_offset, bytes, fb);
+            } else if (F8 && ph != PH_LM) {
+              // e4m3 codes of the tile, then the row exponents of its group right behind them
+              mbar_expect_tx(fb, MEGA_F8_TILE_BYTES + 16);
+              const uint8_t* src = f8.tiles + (int64_t)l * f8.layer_stride + ((int64_t)g0 * tpg + j) * MEGA_F8_TILE_BYTES;
+              if (evf) bulk_g2s_hint(dst, src, MEGA_F8_TILE_BYTES, fb, pol);
+              else bulk_g2s(dst, src, MEGA_F8_TILE_BYTES, fb);
+              bulk_g2s(dst + MEGA_F8_TILE_BYTES, f8.exps + (int64_t)l * f8.exp_stride + (int64_t)(g0 + (int)jk) * 16, 16, fb);
             } else {
               mbar_expect_tx(fb, TILE_BYTES);
               if (evf) bulk_g2s_hint(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb, pol);
@@ -457,6 +494,10 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
             }
             sl += NPW;
             if (sl >= (uint32_t)nslots) { sl -= nslots; ++use; }
+            if (F8) {
+              jks += NPW;
+              while (jks >= (uint32_t)tpg) { jks -= tpg; ++jk; }
+            }
           }
         }
         w.nb += ntiles;
@@ -843,7 +884,42 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
           // batches, so that the tensor pipe starts while the rest of the tile is still being read (shared-memory returns
           // are in order; all 16 ldmatrix in front of the first mma make the two pipes take turns).
           float rA0, rA2;
-          {
+          if (F8 && ph != PH_LM) {
+            // ---- e4m3 tile: [kstep pair][lane][16 B] = this lane's A fragments of two k-steps, converted in registers to the
+            // bf16 bits of code x 2^k_r (rows g and g + 8 of the group: one scale each); same mma sequence as the bf16 tile
+            cur_slot = sl;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
+            const uint32_t ta = ring_u32 + sl * TILE_BYTES + lane * 16;
+            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
+            uint2 b[16];
+#pragma unroll
+            for (int s = 0; s < 16; ++s) b[s] = xp[s * 8];
+            uint4 q[8];
+#pragma unroll
+            for (int s = 0; s < 8; ++s)
+              asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[s].x), "=r"(q[s].y), "=r"(q[s].z), "=r"(q[s].w) : "r"(ta + s * 512));
+            int e0, e1;
+            {
+              const uint32_t ea = ring_u32 + sl * TILE_BYTES + MEGA_F8_TILE_BYTES + (lane >> 2);
+              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e0) : "r"(ea));
+              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e1) : "r"(ea + 8));
+            }
+            release();
+            const float s0 = pow2f(e0), s1 = pow2f(e1);
+            if (!(dflags & 1)) {
+#pragma unroll
+              for (int s = 0; s < 8; ++s) {
+                const uint32_t a0[4] = {e4m3x2_to_bf16x2(q[s].x, s0), e4m3x2_to_bf16x2(q[s].x >> 16, s1),
+                                        e4m3x2_to_bf16x2(q[s].y, s0), e4m3x2_to_bf16x2(q[s].y >> 16, s1)};
+                const uint32_t a1[4] = {e4m3x2_to_bf16x2(q[s].z, s0), e4m3x2_to_bf16x2(q[s].z >> 16, s1),
+                                        e4m3x2_to_bf16x2(q[s].w, s0), e4m3x2_to_bf16x2(q[s].w >> 16, s1)};
+                mma_bf16_16816(acc, a0, b[2 * s].x, b[2 * s].y);
+                mma_bf16_16816(c1, a1, b[2 * s + 1].x, b[2 * s + 1].y);
+              }
+            }
+            rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);
+            rA2 = (acc[2] + c1[2]) + (acc[3] + c1[3]);
+          } else {
             cur_slot = sl;
             float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
             const uint32_t ta = ring_u32 + sl * TILE_BYTES + lane * 16;
@@ -958,6 +1034,15 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
 // ------------------------------------------------------------------ one-time weight re-tiling
 // dst chunk q (16 B) = tile (group, ks) -> [kstep s][matrix m][row r]: rows-half = m & 1, k-half = m >> 1
 // TILE_ROPE: head blocks of hd rows; group gi holds pair rows (i, i + hd/2) for i in 8 consecutive values
+// source row of A-operand row ar (0..15) of group gi
+DTK_DEV int tile_row(int mode, int hd, int gi, int ar) {
+  if (mode == TILE_SEQ) return gi * 16 + ar;
+  if (mode == TILE_ROPE) {
+    const int gph = hd / 16;   // groups per head block
+    return (gi / gph) * hd + ((gi % gph) << 3) + (ar & 7) + (ar >> 3) * (hd / 2);
+  }
+  return (ar < 8) ? 2 * (gi * 8 + ar) : 2 * (gi * 8 + ar - 8) + 1;  // source rows are interleaved (gate, up)
+}
 __global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
                                                      int tpg, bf16* __restrict__ dst) {
   const int64_t q = (int64_t)blockIdx.x * 256 + threadIdx.x;
@@ -968,16 +1053,72 @@ __global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ sr
   const int ks = (int)(tile % tpg), gi = (int)(tile / tpg);
   const int ar = (m & 1) * 8 + r;                      // A-operand row 0..15
   const int col = ks * 256 + s * 16 + (m >> 1) * 8;
-  int row;
-  if (mode == TILE_SEQ) row = gi * 16 + ar;
-  else if (mode == TILE_ROPE) {
-    const int gph = hd / 16;   // groups per head block
-    row = (gi / gph) * hd + ((gi % gph) << 3) + (ar & 7) + (ar >> 3) * (hd / 2);
-  }
-  else row = (ar < 8) ? 2 * (gi * 8 + ar) : 2 * (gi * 8 + ar - 8) + 1;  // source rows are interleaved (gate, up)
+  const int row = tile_row(mode, hd, gi, ar);
   uint4 v = make_uint4(0, 0, 0, 0);
   if (row < N && col < K) v = *reinterpret_cast<const uint4*>(src + (int64_t)row * K + col);
   *reinterpret_cast<uint4*>(dst + q * 8) = v;
+}
+
+// FP8 tiles, step 1: one warp per tile row derives k_r and counts the row's values that are not e4m3 x 2^k_r
+__global__ void __launch_bounds__(256) f8_rows_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
+                                                      int8_t* __restrict__ exps, unsigned int* bad) {
+  const int tr = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (tr >= groups * 16) return;
+  const int row = tile_row(mode, hd, tr >> 4, tr & 15);
+  const bf16* w = src + (int64_t)row * K;
+  float amax = 0.f;
+  if (row < N)
+    for (int i = lane; i < K; i += 32) amax = fmaxf(amax, fabsf(__bfloat162float(w[i])));   // (fmaxf drops NaN: checked below)
+  amax = warp_max(amax);
+  int k = 0;
+  if (amax > 0.f && isfinite(amax)) {
+    int e;
+    const float f = frexpf(amax, &e);   // amax = f 2^e, f in [0.5, 1); 448 = 0.875 2^9: amax <= 448 2^k  <=>  k >= e - 9 (+1 if f > 0.875)
+    k = max(e - 9 + (f > 0.875f ? 1 : 0), -117);
+  }
+  unsigned int nbad = 0;
+  if (row < N) {
+    const float inv = pow2f(-k);
+    for (int i = lane; i < K; i += 32) {
+      const float v = __bfloat162float(w[i]) * inv;
+      if (!(e4m3x2_to_float2(float2_to_e4m3x2(v, 0.f)).x == v)) ++nbad;   // NaN, inf and values off the e4m3 grid
+    }
+  }
+  nbad = __reduce_add_sync(0xffffffffu, nbad);
+  if (lane == 0) {
+    exps[tr] = (int8_t)k;
+    if (nbad) atomicAdd(bad, nbad);
+  }
+}
+// FP8 tiles, step 2: one thread per 16-byte chunk (tile, kstep pair p, lane) = e4m3 codes of the lane's A fragments
+__global__ void __launch_bounds__(256) f8_tile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
+                                                      int tpg, const int8_t* __restrict__ exps, uint8_t* __restrict__ dst) {
+  const int64_t q = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (q >= (int64_t)groups * tpg * 256) return;
+  const int lane = (int)(q & 31), p = (int)((q >> 5) & 7);
+  const int64_t tile = q >> 8;
+  const int ks = (int)(tile % tpg), gi = (int)(tile / tpg);
+  uint32_t out[4];
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {   // word h: k-step 2p + (h >> 1), fragments 2 (h & 1) and 2 (h & 1) + 1
+    uint32_t word = 0;
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int m = 2 * (h & 1) + u;                        // fragment: rows-half m & 1, k-half m >> 1
+      const int ar = (m & 1) * 8 + (lane >> 2);
+      const int row = tile_row(mode, hd, gi, ar);
+      const int col = ks * 256 + (2 * p + (h >> 1)) * 16 + (m >> 1) * 8 + 2 * (lane & 3);
+      uint32_t codes = 0;
+      if (row < N && col < K) {   // K % 8 == 0: col + 1 < K too
+        const float inv = pow2f(-exps[gi * 16 + ar]);
+        const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(src + (int64_t)row * K + col));
+        codes = float2_to_e4m3x2(v.x * inv, v.y * inv);
+      }
+      word |= codes << (16 * u);
+    }
+    out[h] = word;
+  }
+  *reinterpret_cast<uint4*>(dst + q * 16) = make_uint4(out[0], out[1], out[2], out[3]);
 }
 
 }  // namespace
@@ -996,6 +1137,17 @@ cudaError_t launch_retile(const bf16* src, int N, int K, int mode, int hd, bf16*
   mega_tiled_elems(N, K, mode, &groups, &tpg);
   const int64_t chunks = (int64_t)groups * tpg * 512;
   retile_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(src, N, K, mode, hd, groups, tpg, dst);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_retile_f8(const bf16* src, int N, int K, int mode, int hd, uint8_t* dst, int8_t* exps, unsigned int* bad,
+                             cudaStream_t s) {
+  if ((K & 7) || (mode == TILE_ROPE && ((hd != 64 && hd != 128) || N % hd))) return cudaErrorInvalidValue;
+  int groups, tpg;
+  mega_tiled_elems(N, K, mode, &groups, &tpg);
+  f8_rows_kernel<<<(unsigned)((groups * 16 + 7) / 8), 256, 0, s>>>(src, N, K, mode, hd, groups, exps, bad);
+  const int64_t chunks = (int64_t)groups * tpg * 256;
+  f8_tile_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(src, N, K, mode, hd, groups, tpg, exps, dst);
   return cudaGetLastError();
 }
 
@@ -1037,8 +1189,11 @@ cudaError_t launch_decode_mega(const MegaArgs& a, int grid, cudaStream_t s, uint
   const int smem = mega_smem_bytes(a);
   const bool dbgk = a.dbg != nullptr || a.dbg2 != nullptr || a.dbg_flags != 0;
   const void* fn;
-  if (a.hd == 128) fn = dbgk ? (const void*)decode_mega_kernel<true, 128> : (const void*)decode_mega_kernel<false, 128>;
-  else if (a.hd == 64) fn = dbgk ? (const void*)decode_mega_kernel<true, 64> : (const void*)decode_mega_kernel<false, 64>;
+  const bool f8 = a.f8[0].tiles != nullptr;
+  if (a.hd == 128 && !f8) fn = dbgk ? (const void*)decode_mega_kernel<true, 128, false> : (const void*)decode_mega_kernel<false, 128, false>;
+  else if (a.hd == 64 && !f8) fn = dbgk ? (const void*)decode_mega_kernel<true, 64, false> : (const void*)decode_mega_kernel<false, 64, false>;
+  else if (a.hd == 128) fn = dbgk ? (const void*)decode_mega_kernel<true, 128, true> : (const void*)decode_mega_kernel<false, 128, true>;
+  else if (a.hd == 64) fn = dbgk ? (const void*)decode_mega_kernel<true, 64, true> : (const void*)decode_mega_kernel<false, 64, true>;
   else return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;

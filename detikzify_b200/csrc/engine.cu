@@ -248,7 +248,10 @@ struct dtk_engine {
   SampleArgs gen_sample{};
   unsigned long long* d_bar = nullptr;  // [0] counter, [1] epoch base
   unsigned int* d_head_cnt = nullptr;
-  bf16* d_tiled = nullptr;             // decode-side re-tiled copy of the decoder matrices
+  bf16* d_tiled = nullptr;             // decode-side re-tiled copy of the four layer matrices (bf16 mode)
+  bf16* d_tiled_lm = nullptr;          // ... and of the lm_head (always bf16)
+  uint8_t* d_tiled8 = nullptr;         // FP8 mode (option "decode_fp8"): e4m3 tiles, row exponents and check counters
+  int decode_fp8 = 0;
   unsigned long long* d_tagged = nullptr;  // {fp32 value, phase tag} cross-CTA activation words of the persistent kernel
   long long* d_dbg = nullptr;           // phase timestamps of the persistent kernel (option mega_debug)
   long long* d_dbg2 = nullptr;          // per-tile clock trace of one layer (option mega_trace_layer)
@@ -554,6 +557,76 @@ bf16* kv_layer(dtk_engine* eng, int slot, int layer) {
   return eng->kv + (int64_t)slot * eng->kv_slot_stride + (int64_t)layer * eng->kv_layer_stride;
 }
 
+// Decode-side tiles of the four layer matrices from the arena: bf16 (MegaMat::base) or FP8 (MegaArgs::f8, which requires
+// every row of every layer matrix to be e4m3 x 2^k_r). The new tiles are built and checked in a buffer of their own; only
+// then are they swapped in and the other format's tiles freed, so a failure leaves the engine as it was.
+int mega_layer_tiles(dtk_engine* eng, bool fp8) {
+  static const char* names[4] = {"wqkv", "wo", "wgu", "wd"};
+  const dtk_config& c = eng->cfg;
+  MegaArgs& m = eng->mega;
+  const int hd = c.head_dim, L = c.layers;
+  const int64_t esz = fp8 ? 1 : 2;   // bytes per weight of a tile
+  int64_t per_layer = 0, off[4], exp_layer = 0, eoff[4];
+  for (int i = 0; i < 4; ++i) {
+    off[i] = per_layer;
+    per_layer += (int64_t)m.mat[i].groups * m.mat[i].tpg * MEGA_TILE_ELEMS * esz;
+    eoff[i] = exp_layer;
+    exp_layer += (int64_t)m.mat[i].groups * 16;
+  }
+  const int64_t tiles_bytes = per_layer * L, exp0 = tiles_bytes, bad0 = (exp0 + exp_layer * L + 255) / 256 * 256;
+  const int64_t total = fp8 ? bad0 + 4 * (int64_t)L * 4 : tiles_bytes;
+  DTK_CK(cudaDeviceSynchronize());   // the arena is written; no launch reads the current tiles any more
+  uint8_t* buf = nullptr;
+  DTK_ALLOC(buf, total);
+  unsigned int* bad = reinterpret_cast<unsigned int*>(buf + bad0);
+  cudaError_t e = fp8 ? cudaMemset(bad, 0, 4 * (size_t)L * sizeof(unsigned int)) : cudaSuccess;
+  for (int l = 0; l < L && e == cudaSuccess; ++l)
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) {
+      const MegaMat& mm = m.mat[i];
+      const bf16* src = W(eng, LN("dec.L", l, names[i]));
+      uint8_t* dst = buf + (int64_t)l * per_layer + off[i];
+      e = fp8 ? launch_retile_f8(src, mm.N, mm.K, mm.mode, hd, dst, reinterpret_cast<int8_t*>(buf + exp0 + (int64_t)l * exp_layer + eoff[i]),
+                                 bad + l * 4 + i, 0)
+              : launch_retile(src, mm.N, mm.K, mm.mode, hd, reinterpret_cast<bf16*>(dst), 0);
+    }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  std::vector<unsigned int> nbad(fp8 ? 4 * L : 0);
+  if (e == cudaSuccess && fp8) e = cudaMemcpy(nbad.data(), bad, nbad.size() * sizeof(unsigned int), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) {
+    cudaFree(buf);
+    eng->err = std::string("decode tiles: ") + cudaGetErrorString(e);
+    return DTK_ERR_CUDA;
+  }
+  for (size_t k = 0; k < nbad.size(); ++k)
+    if (nbad[k]) {
+      cudaFree(buf);
+      eng->err = "invalid argument: decode_fp8: layer " + std::to_string(k / 4) + " " + names[k % 4] + " holds " +
+                 std::to_string(nbad[k]) + " values that are not an e4m3 value times a power-of-two row scale (quantize the "
+                 "weights first: load(..., quantize=\"fp8\"))";
+      return DTK_ERR_INVALID;
+    }
+  cudaFree(eng->d_tiled);
+  cudaFree(eng->d_tiled8);
+  eng->d_tiled = fp8 ? nullptr : reinterpret_cast<bf16*>(buf);
+  eng->d_tiled8 = fp8 ? buf : nullptr;
+  for (int i = 0; i < 4; ++i) {
+    m.mat[i].base = fp8 ? nullptr : reinterpret_cast<const bf16*>(buf + off[i]);
+    m.mat[i].layer_stride = fp8 ? 0 : per_layer / 2;
+    m.f8[i] = fp8 ? MegaF8{buf + off[i], reinterpret_cast<const int8_t*>(buf + exp0 + eoff[i]), per_layer, exp_layer} : MegaF8{};
+  }
+  eng->decode_fp8 = fp8 ? 1 : 0;
+  return DTK_OK;
+}
+
+// weight bytes one batch-1 persistent decode token streams: the four layer matrices (bf16, or e4m3 codes plus one exponent
+// per row), the lm_head in bf16
+uint64_t decode_weight_bytes(const dtk_config& c, bool fp8) {
+  const uint64_t H = c.hidden, I = c.inter, V = c.vocab, qd = (uint64_t)c.heads * c.head_dim, kd = (uint64_t)c.kv_heads * c.head_dim;
+  const uint64_t layer_w = (uint64_t)c.layers * ((qd + 2 * kd) * H + H * qd + 3 * H * I);
+  const uint64_t layer_rows = (uint64_t)c.layers * ((qd + 2 * kd) + H + 2 * I + H);
+  return (fp8 ? layer_w + layer_rows : 2 * layer_w) + 2 * V * H;
+}
+
 int nsplit_for(const dtk_config& c, int B) {
   int n = (2 * 132 + c.heads * B - 1) / (c.heads * B);   // two CTAs on each of the H100's 132 SMs
   if (n < 1) n = 1;
@@ -823,31 +896,28 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
       m.embed = W(eng, "dec.embed"); m.final_norm = W(eng, "dec.norm");
       m.norm1_0 = W(eng, "dec.L0.norm1"); m.norm2_0 = W(eng, "dec.L0.norm2");
       m.norm_stride = c.layers > 1 ? (int64_t)(W(eng, "dec.L1.norm1") - W(eng, "dec.L0.norm1")) : 0;
-      // decode-side tiled weight copy (one-time, on device): [layer][qkv | o | gu | down] ... [lm_head]
+      // decode-side tiled weight copy (one-time, on device): [layer][qkv | o | gu | down] (mega_layer_tiles), [lm_head]
       const int qkvN = (int)((c.heads + 2 * c.kv_heads) * HD);
-      struct Spec { MegaMat* mm; const char* name; int N, K, mode; } specs[4] = {
-          {&m.mat[0], "wqkv", qkvN, c.hidden, TILE_ROPE}, {&m.mat[1], "wo", c.hidden, (int)qd, TILE_SEQ},
-          {&m.mat[2], "wgu", 2 * c.inter, c.hidden, TILE_GLU}, {&m.mat[3], "wd", c.hidden, c.inter, TILE_SEQ}};
-      int64_t per_layer = 0, off[4];
-      for (int i = 0; i < 4; ++i) {
-        off[i] = per_layer;
-        per_layer += mega_tiled_elems(specs[i].N, specs[i].K, specs[i].mode, &specs[i].mm->groups, &specs[i].mm->tpg);
-      }
-      const int64_t lm_elems = mega_tiled_elems(c.vocab, c.hidden, TILE_SEQ, &m.mat[4].groups, &m.mat[4].tpg);
-      DTK_ALLOC(eng->d_tiled, per_layer * c.layers + lm_elems);
+      struct Spec { MegaMat* mm; int N, K, mode; } specs[4] = {
+          {&m.mat[0], qkvN, c.hidden, TILE_ROPE}, {&m.mat[1], c.hidden, (int)qd, TILE_SEQ},
+          {&m.mat[2], 2 * c.inter, c.hidden, TILE_GLU}, {&m.mat[3], c.hidden, c.inter, TILE_SEQ}};
       for (int i = 0; i < 4; ++i) {
         MegaMat& mm = *specs[i].mm;
-        mm.base = eng->d_tiled + off[i]; mm.layer_stride = per_layer; mm.N = specs[i].N; mm.K = specs[i].K; mm.mode = specs[i].mode;
-        for (int l = 0; l < c.layers; ++l)
-          DTK_CK(launch_retile(W(eng, LN("dec.L", l, specs[i].name)), specs[i].N, specs[i].K, specs[i].mode, c.head_dim,
-                               eng->d_tiled + (int64_t)l * per_layer + off[i], 0));
+        mega_tiled_elems(specs[i].N, specs[i].K, specs[i].mode, &mm.groups, &mm.tpg);
+        mm.N = specs[i].N; mm.K = specs[i].K; mm.mode = specs[i].mode;
       }
+      const int64_t lm_elems = mega_tiled_elems(c.vocab, c.hidden, TILE_SEQ, &m.mat[4].groups, &m.mat[4].tpg);
       for (int i = 0; i < 5; ++i) {
         m.mat[i].per = (m.mat[i].groups + grid - 1) / grid;
         m.mat[i].nact = (m.mat[i].groups + m.mat[i].per - 1) / m.mat[i].per;
       }
-      m.mat[4].base = eng->d_tiled + per_layer * c.layers; m.mat[4].layer_stride = 0; m.mat[4].N = c.vocab; m.mat[4].K = c.hidden; m.mat[4].mode = TILE_SEQ;
-      DTK_CK(launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, c.head_dim, eng->d_tiled + per_layer * c.layers, 0));
+      {
+        const int r = mega_layer_tiles(eng, false);
+        if (r != DTK_OK) return r;
+      }
+      DTK_ALLOC(eng->d_tiled_lm, lm_elems);
+      m.mat[4].base = eng->d_tiled_lm; m.mat[4].layer_stride = 0; m.mat[4].N = c.vocab; m.mat[4].K = c.hidden; m.mat[4].mode = TILE_SEQ;
+      DTK_CK(launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, c.head_dim, eng->d_tiled_lm, 0));
       m.tok = eng->d_tok; m.pos = eng->d_pos; m.slots = eng->d_slots; m.share_slot = eng->d_share_slot; m.share_len = eng->d_share_len;
       m.kv = eng->kv; m.kv_slot_stride = eng->kv_slot_stride; m.kv_layer_stride = eng->kv_layer_stride;
       m.kv_v_offset = eng->kv_v_offset; m.rope_cs = eng->rope_cs;
@@ -890,7 +960,7 @@ int dtk_destroy(dtk_engine* eng) {
   for (auto& g : eng->vit_graphs) cudaGraphExecDestroy(g.second.exec);
   void* ptrs[] = {eng->v_pix_in, eng->v_tok_out, eng->v_pool_out, eng->v_vt, eng->kv, eng->rope_cs, eng->p_x, eng->p_qkv, eng->p_xn, eng->p_q, eng->p_att, eng->p_h, eng->d_x, eng->d_q,
                   eng->d_att, eng->d_h, eng->d_logits, eng->d_scratch, eng->d_part_o, eng->d_part_ml, eng->d_counters,
-                  eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
+                  eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tiled_lm, eng->d_tiled8, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
                   eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt};
   for (void* p : ptrs) if (p) cudaFree(p);
   dtk_adapter_detach(eng);
@@ -1597,6 +1667,12 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
     eng->mega_variant = (int)value;
     return DTK_OK;
   }
+  if (std::strcmp(key, "decode_fp8") == 0) {  // batch-1 persistent decode streams the layer matrices as e4m3 (1) or bf16 (0) tiles
+    DTK_REQUIRE(value == 0 || value == 1, "decode_fp8 must be 0 or 1");
+    DTK_REQUIRE(eng->mega_ok, "decode_fp8: the persistent decode kernel is unavailable on this device");
+    if ((int)value == eng->decode_fp8) return DTK_OK;
+    return mega_layer_tiles(eng, value == 1);
+  }
   if (std::strcmp(key, "mega_nslots") == 0) {  // dev: smaller ring (8 / 16) for A/B runs of the stream's depth
     eng->mega_nslots = (int)value;
     return DTK_OK;
@@ -1619,6 +1695,8 @@ int dtk_get_option(dtk_engine* eng, const char* key, int64_t* value) {
   if (std::strcmp(key, "mega_flags") == 0) { *value = eng->mega_flags; return DTK_OK; }
   if (std::strcmp(key, "mega_debug") == 0) { *value = eng->mega_debug; return DTK_OK; }
   if (std::strcmp(key, "mega_variant") == 0) { *value = eng->mega_variant; return DTK_OK; }
+  if (std::strcmp(key, "decode_fp8") == 0) { *value = eng->decode_fp8; return DTK_OK; }
+  if (std::strcmp(key, "decode_weight_bytes") == 0) { *value = (int64_t)decode_weight_bytes(eng->cfg, eng->decode_fp8 != 0); return DTK_OK; }
   eng->err = std::string("unknown option ") + key;
   return DTK_ERR_INVALID;
 }

@@ -230,6 +230,16 @@ struct MegaMat {
   int per, nact;          // work split over the grid (host-computed: no division in the kernel): per = ceil(groups / grid) groups per participating CTA, nact = ceil(groups / per) participants
   int mode;
 };
+// FP8 decode tiles (launch_retile_f8): each bf16 row r of a layer matrix is e4m3 code x 2^k_r. A tile holds the codes of
+// the same 16 rows x 256 k as the bf16 tile, 4 KB in mma A-fragment order ([kstep pair 8][lane 32][kstep 2][fragment 4]
+// [2 codes]: one 16-byte shared load per lane and kstep pair); exps[group][16] holds k_r of the group's tile rows.
+constexpr int MEGA_F8_TILE_BYTES = 4096;
+struct MegaF8 {
+  const uint8_t* tiles;   // layer 0
+  const int8_t* exps;     // layer 0
+  int64_t layer_stride;   // bytes between layers of tiles
+  int64_t exp_stride;     // bytes between layers of exps
+};
 struct MegaArgs {
   int H, I, L, heads, kv_heads, V, max_len;
   int hd;                                                     // decoder head_dim, 64 or 128 (mega_configure)
@@ -261,6 +271,8 @@ struct MegaArgs {
   long long* dbg;                                             // optional: [grid][5L+1][4] globaltimer stamps (null = off)
   long long* dbg2;                                            // optional: [grid][MEGA_DBG2_ROWS][4] clock64 per-tile trace of layer dbg_layer
   int dbg_layer;
+  // FP8 decoder weights (option "decode_fp8"; null tiles = bf16): e4m3 tiles of the four layer matrices, same order as mat[0..3]
+  MegaF8 f8[4];
 };
 int mega_smem_bytes(const MegaArgs& a);
 cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int hd, int max_smem_optin, int num_sms, int* grid_out);
@@ -268,6 +280,10 @@ cudaError_t launch_decode_mega(const MegaArgs& a, int grid, cudaStream_t s, uint
 // one-time re-tiling of a row-major [N, K] (ld = K) matrix into the decode layout (hd: head_dim of TILE_ROPE)
 int64_t mega_tiled_elems(int N, int K, int mode, int* groups, int* tpg);
 cudaError_t launch_retile(const bf16* src, int N, int K, int mode, int hd, bf16* dst, cudaStream_t s);
+// the same matrix into FP8 tiles: derives each row's k_r (the smallest k with max |w| <= 448 * 2^k, at least -117; 0 for a
+// row of zeros) into exps and adds to *bad the number of values that are not an e4m3 value times 2^k_r (those tiles are junk)
+cudaError_t launch_retile_f8(const bf16* src, int N, int K, int mode, int hd, uint8_t* dst, int8_t* exps, unsigned int* bad,
+                             cudaStream_t s);
 
 // device image preprocessing (Pillow-exact 8-bit bicubic resize + rescale + normalise): rgb uint8 [h, w, 3] -> fp32 [3, S, S]
 cudaError_t launch_image_preprocess(const uint8_t* rgb, int h, int w, int S, const int* bounds_h, const int* coef_h, int ksize_h,

@@ -97,7 +97,8 @@ def build_processor(cfg: DetikzifyConfig, tokenizer=None) -> DetikzifyProcessor:
 def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bool = False, *,
          random_init_weights: Optional[bool] = None, seed: int = 0, state_dict: Optional[Dict[str, torch.Tensor]] = None,
          config: Optional[DetikzifyConfig] = None, max_seqs: int = 2, max_batch: int = 1, broadcast: bool = False,
-         prefix_slots: Optional[int] = None, device_init: bool = False, vision_tower: Optional[str] = None, **kwargs):
+         prefix_slots: Optional[int] = None, device_init: bool = False, vision_tower: Optional[str] = None,
+         quantize: Optional[str] = None, **kwargs):
     """Returns ``(model, processor)``.
 
     ``max_seqs`` KV slots are preallocated (0.40 GB each for ds-1.3b at 2k context); ``generate()`` keeps a prefix cache
@@ -109,10 +110,20 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
 
     ``broadcast=True`` (multi-GPU, one process per GPU): only rank 0 materialises the weights; the
     packed arena is sent with ONE ``torch.distributed.broadcast`` over NCCL (SURVEY.md §8e).
+
+    ``quantize="fp8"``: weight-only e4m3 quantization of the decoder-layer matrices (q/k/v/o, gate/up, down) with one
+    power-of-two scale per output row (``detikzify_b200.quant``). The arena holds the dequantized values, so every path
+    computes the same quantized model, and batch-1 decode streams the layer matrices as e4m3 (about half the bytes).
+    Embeddings, norms, lm_head, projector, vision tower and KV cache stay bf16. ``None`` (default) keeps the weights as
+    they are.
     """
-    from ..engine import pack_arena, to_c_config
+    from ..engine import pack_arena, to_c_config, weight_table
+    from ..quant import quantize_arena_fp8
     from .. import _lib
     import ctypes as C
+
+    if quantize not in (None, "fp8"):
+        raise ValueError(f"quantize must be None or 'fp8', got {quantize!r}")
 
     is_dir = isinstance(model_name_or_path, str) and os.path.isdir(model_name_or_path)
     cfg = config
@@ -155,6 +166,8 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
                 sd["model.mm_projector." + k.split(".")[-1]] = v
         arena = pack_arena(cfg, sd)
         del sd
+    if rank0 and quantize == "fp8":   # before the broadcast: every rank holds the same bytes
+        quantize_arena_fp8(arena, weight_table(to_c_config(cfg)))
     if broadcast:
         import torch.distributed as dist
         lib = _lib.load_library()
@@ -165,6 +178,8 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
 
     model = DetikzifyForCausalLM(cfg, arena, device=device, dtype=dtype, max_seqs=max_seqs, max_batch=max_batch,
                                  prefix_slots=prefix_slots)
+    if quantize == "fp8":
+        model.engine.set_option("decode_fp8", 1)
     tokenizer = _load_tokenizer(model_name_or_path, cfg) if is_dir else None
     return model, build_processor(cfg, tokenizer)
 

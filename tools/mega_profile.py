@@ -1,12 +1,15 @@
 """Phase-level timeline of the persistent decode kernel across all CTAs (dev tool).
-Usage: python tools/mega_profile.py [model] [ctx] [trace.pt]  (the trace goes to the temporary directory by default)."""
+Usage: python tools/mega_profile.py [--fp8] [model] [ctx] [trace.pt]  (the trace goes to the temporary directory by default;
+--fp8: weights quantized as load(..., quantize="fp8") does, decode on the FP8 layer tiles)."""
 import ctypes as C, os, sys, tempfile
 import torch
 sys.path.insert(0, ".")
 from detikzify_b200.model import load
+fp8 = "--fp8" in sys.argv
+sys.argv = [a for a in sys.argv if a != "--fp8"]
 name = sys.argv[1] if len(sys.argv) > 1 else "nllg/detikzify-ds-1.3b"
 ctx = int(sys.argv[2]) if len(sys.argv) > 2 else 1000
-model, _ = load(name, device_map=0)
+model, _ = load(name, device_map=0, quantize="fp8" if fp8 else None)
 eng, cfg = model.engine, model.config
 slot = eng.seq_alloc()
 g = torch.Generator().manual_seed(1)
