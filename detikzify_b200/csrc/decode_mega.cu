@@ -35,9 +35,8 @@
 // in the kernel tail). DESIGN.md section 4 describes the design.
 //
 // Replaces the per-token HF eager path (modeling_llama.py:303-333, ~900 launches per token).
-#include <cuda_fp16.h>
-
 #include "common.cuh"
+#include "fp8.cuh"
 #include "launch.h"
 
 namespace dtk {
@@ -108,26 +107,6 @@ DTK_DEV uint64_t policy_evict_first() {
   return pol;
 }
 DTK_DEV void consumer_sync() { asm volatile("bar.sync 1, %0;\n" ::"n"(CONSUMER_THREADS) : "memory"); }
-
-// ------------------------------------------------------------------ e4m3 codes
-// two e4m3 codes (low 16 bits of v: low byte = first element) -> their values (exact in fp32)
-DTK_DEV float2 e4m3x2_to_float2(uint32_t v) {
-  uint32_t h;
-  asm("{\n\t.reg .b16 t;\n\tcvt.u16.u32 t, %1;\n\tcvt.rn.f16x2.e4m3x2 %0, t;\n\t}\n" : "=r"(h) : "r"(v));
-  return __half22float2(*reinterpret_cast<const __half2*>(&h));
-}
-// the bf16 pair of an A fragment: two codes times the row scale 2^k_r (exact: the product is a bf16 value)
-DTK_DEV uint32_t e4m3x2_to_bf16x2(uint32_t v, float scale) {
-  const float2 f = e4m3x2_to_float2(v);
-  return pack_bf16x2(f.x * scale, f.y * scale);
-}
-// (a, b) -> two e4m3 codes (round to nearest even, saturating), a in the low byte
-DTK_DEV uint32_t float2_to_e4m3x2(float a, float b) {
-  uint16_t d;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;\n" : "=h"(d) : "f"(b), "f"(a));
-  return d;
-}
-DTK_DEV float pow2f(int k) { return __uint_as_float((uint32_t)(k + 127) << 23); }   // k in [-126, 127]
 
 // ------------------------------------------------------------------ tagged activation words
 // Every activation value that crosses CTAs (residual stream, q, the new key/value row, attention partials and output,
@@ -1032,17 +1011,8 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
 }
 
 // ------------------------------------------------------------------ one-time weight re-tiling
-// dst chunk q (16 B) = tile (group, ks) -> [kstep s][matrix m][row r]: rows-half = m & 1, k-half = m >> 1
-// TILE_ROPE: head blocks of hd rows; group gi holds pair rows (i, i + hd/2) for i in 8 consecutive values
-// source row of A-operand row ar (0..15) of group gi
-DTK_DEV int tile_row(int mode, int hd, int gi, int ar) {
-  if (mode == TILE_SEQ) return gi * 16 + ar;
-  if (mode == TILE_ROPE) {
-    const int gph = hd / 16;   // groups per head block
-    return (gi / gph) * hd + ((gi % gph) << 3) + (ar & 7) + (ar >> 3) * (hd / 2);
-  }
-  return (ar < 8) ? 2 * (gi * 8 + ar) : 2 * (gi * 8 + ar - 8) + 1;  // source rows are interleaved (gate, up)
-}
+// dst chunk q (16 B) = tile (group, ks) -> [kstep s][matrix m][row r]: rows-half = m & 1, k-half = m >> 1; rows in the
+// order of tile_row (fp8.cuh)
 __global__ void __launch_bounds__(256) retile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
                                                      int tpg, bf16* __restrict__ dst) {
   const int64_t q = (int64_t)blockIdx.x * 256 + threadIdx.x;

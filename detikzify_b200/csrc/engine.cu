@@ -605,6 +605,9 @@ int mega_layer_tiles(dtk_engine* eng, bool fp8) {
                  "weights first: load(..., quantize=\"fp8\"))";
       return DTK_ERR_INVALID;
     }
+  // captured batched decode steps bake in the tile pointers of the old format, which are freed here
+  for (auto& g : eng->graphs) cudaGraphExecDestroy(g.second);
+  eng->graphs.clear();
   cudaFree(eng->d_tiled);
   cudaFree(eng->d_tiled8);
   eng->d_tiled = fp8 ? nullptr : reinterpret_cast<bf16*>(buf);
@@ -671,10 +674,20 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
     // Activations are rounded to bf16 GEMM operands exactly as in prefill
     // (fp32 residual stream, fp32 accumulation); RoPE / KV append / attention are per row (slot, position).
     const int qkvd = qd + 2 * kd;
-    auto gemm = [&](const bf16* A, int K, const bf16* Wm, int N, const float* resid, int glu, float* o32, bf16* o16, int ldo) {
+    // decode_fp8: the four layer matrices (mat = 0..3 of layer l) stream from the FP8 decode tiles on the swapped-operand
+    // tile, with the result bits of the bf16 arena. B >= 64 runs the dense bf16 tile, and the lm_head stays bf16.
+    const bool fp8 = eng->decode_fp8 != 0 && B < 64;
+    auto gemm = [&](const bf16* A, int K, const bf16* Wm, int N, const float* resid, int glu, float* o32, bf16* o16, int ldo,
+                    int l = 0, int mat = -1) {
       GemmArgs g{};
       g.A = A; g.lda = K; g.W = Wm; g.ldw = K; g.M = B; g.N = N; g.K = K;
       g.resid = resid; g.ldr = ldo; g.glu = glu; g.out_f32 = o32; g.out_bf16 = o16; g.ldo = ldo;
+      if (fp8 && mat >= 0) {
+        const MegaMat& mm = eng->mega.mat[mat];
+        const MegaF8& t = eng->mega.f8[mat];
+        const GemmF8 w{t.tiles + l * t.layer_stride, t.exps + l * t.exp_stride, mm.groups, mm.tpg, mm.mode, HD};
+        return launch_gemm_swap_f8(g, w, s, lc);
+      }
       return launch_gemm(g, s, lc);
     };
     // Shared-prefix ("cascade") attention: when every row borrows the same prefix from one slot (MCTS rollouts of a figure),
@@ -688,7 +701,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
     const int csplit = cas ? (ctiles_all + ctile - 1) / ctile : 0;
     for (int l = 0; l < c.layers; ++l) {
       DTK_CK(launch_rmsnorm(eng->d_x, H, W(eng, LN("dec.L", l, "norm1")), c.rms_eps, B, H, eng->p_xn, s, lc));
-      DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wqkv")), qkvd, nullptr, 0, eng->p_qkv, nullptr, qkvd));
+      DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wqkv")), qkvd, nullptr, 0, eng->p_qkv, nullptr, qkvd, l, 0));
       DTK_CK(launch_rope_kv_decode(eng->p_qkv, B, eng->d_slots, eng->d_pos, c.heads, c.kv_heads, eng->rope_cs, eng->d_q,
                                    kv_layer(eng, 0, l), eng->kv_slot_stride, eng->kv_v_offset, c.max_len, HD, s, lc, cas ? eng->p_q : nullptr));
       if (cas) {
@@ -713,10 +726,10 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
         if (cas) { a.key_begin = eng->cas_len; a.np = nsplit + csplit; }
         DTK_CK(launch_decode_attn(a, s, lc));
       }
-      DTK_CK(gemm(eng->p_att, qd, W(eng, LN("dec.L", l, "wo")), H, eng->d_x, 0, eng->d_x, nullptr, H));
+      DTK_CK(gemm(eng->p_att, qd, W(eng, LN("dec.L", l, "wo")), H, eng->d_x, 0, eng->d_x, nullptr, H, l, 1));
       DTK_CK(launch_rmsnorm(eng->d_x, H, W(eng, LN("dec.L", l, "norm2")), c.rms_eps, B, H, eng->p_xn, s, lc));
-      DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wgu")), 2 * I, nullptr, 1, nullptr, eng->p_h, I));
-      DTK_CK(gemm(eng->p_h, I, W(eng, LN("dec.L", l, "wd")), H, eng->d_x, 0, eng->d_x, nullptr, H));
+      DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wgu")), 2 * I, nullptr, 1, nullptr, eng->p_h, I, l, 2));
+      DTK_CK(gemm(eng->p_h, I, W(eng, LN("dec.L", l, "wd")), H, eng->d_x, 0, eng->d_x, nullptr, H, l, 3));
     }
     DTK_CK(launch_rmsnorm(eng->d_x, H, W(eng, "dec.norm"), c.rms_eps, B, H, eng->p_xn, s, lc));
     DTK_CK(gemm(eng->p_xn, H, W(eng, "dec.lm_head"), c.vocab, nullptr, 0, logits, nullptr, c.vocab));

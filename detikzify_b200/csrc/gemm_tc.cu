@@ -14,6 +14,7 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "fp8.cuh"
 #include "launch.h"
 #include "wgmma.cuh"
 
@@ -36,6 +37,8 @@ DTK_DEV void wgmma_tile(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { 
 DTK_DEV void wgmma_tile(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n256k16_ss(d, a, b, acc); }
 DTK_DEV void wgmma_tile(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n32k16_ss(d, a, b, acc); }
 DTK_DEV void wgmma_tile(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n64k16_ss(d, a, b, acc); }
+DTK_DEV void wgmma_tile_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_m64n32k16_rs(d, a, b, acc); }
+DTK_DEV void wgmma_tile_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t acc) { wgmma_m64n64k16_rs(d, a, b, acc); }
 
 // 0.5 x (1 + tanh(u)) = x * sigmoid(2u): two MUFU ops instead of the libm tanhf (error ~1e-7 relative, far below bf16 output rounding)
 DTK_DEV float gelu_tanh_fast(float x) {
@@ -230,13 +233,22 @@ DTK_DEV float ld_dsmem(uint32_t cluster_addr) {
 // streams a contiguous K range into its own accumulator, ranks > 0 park their fp32 partial tile in their shared memory
 // and rank 0 adds them IN RANK ORDER through distributed shared memory (deterministic) and runs the epilogue. No workspace in
 // HBM, no atomics. Two CTAs per SM (5-stage rings) keep ~200 KB of weights in flight per SM.
+//
+// F8 = true: the weights are FP8 decode tiles (GemmF8; mapW unused). The CTA's 128 rows are the 8 row groups
+// 8 (blockIdx / nsplit) .. + 7, warp q's 16 accumulator rows = group q in the tiles' row permutation (tile_row). A 64-wide
+// k-block kb of one group is 1 KB of contiguous codes ([kstep pair 2][lane 32][16 B] at byte (kb % 4) KB of 256-k tile
+// kb / 4): the producer bulk-copies one per group that exists, each lane loads its 2 x 16 B, rebuilds the bf16 bits of
+// code x 2^k_r for rows g and g + 8 (fp8.cuh) and issues the wgmma with A from registers. Same k-blocks, split-K cuts,
+// k16 order and rank-order reduction as the bf16 tile, so a matrix holding exactly those values gives the same bits.
+// A stage carries half the weight bytes, so the ring is deeper (TSTAGES as deep as two CTAs per SM allow).
 constexpr int STHREADS = 288;   // two consumer warpgroups + the producer warp
-template <int NB, int TSTAGES>
+template <int NB, int TSTAGES, bool F8 = false>
 __global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_constant__ CUtensorMap mapW,
                                                                   const __grid_constant__ CUtensorMap mapX, const GemmArgs p,
-                                                                  const int nsplit) {
+                                                                  const int nsplit, const GemmF8 f8) {
+  constexpr int W_BYTES = F8 ? TBM * TBK : A_BYTES;   // e4m3 codes or bf16 weights of one k-block
   constexpr int X_BYTES = NB * TBK * 2;
-  constexpr int STAGE_BYTES = A_BYTES + X_BYTES;
+  constexpr int STAGE_BYTES = W_BYTES + X_BYTES;
   constexpr int NACC = NB / 2;
   static_assert(NACC * 256 * 4 <= TSTAGES * STAGE_BYTES, "the partial tile is parked in the drained ring");
   extern __shared__ uint8_t smem_raw[];
@@ -256,13 +268,28 @@ __global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_
 
   if (warp == 8) {
     if (lane == 0) {
-      for (int kt = 0; kt < KT; ++kt) {
-        const int s = kt % TSTAGES, use = kt / TSTAGES;
-        if (use > 0) mbar_wait(empty0 + 8 * s, (use - 1) & 1);
-        const uint32_t sw = sbase + s * STAGE_BYTES, sx = sw + A_BYTES;
-        mbar_expect_tx(full0 + 8 * s, STAGE_BYTES);
-        tma_load_2d(sw, &mapW, (kt0 + kt) * TBK, n0, full0 + 8 * s);
-        tma_load_2d(sx, &mapX, (kt0 + kt) * TBK, 0, full0 + 8 * s);
+      if constexpr (F8) {
+        const int g0 = n0 / 16, ng = min(8, f8.groups - g0);   // groups past the matrix's last are neither copied nor stored
+        const int64_t gstride = (int64_t)f8.tpg * MEGA_F8_TILE_BYTES;
+        const uint8_t* src0 = f8.tiles + g0 * gstride;
+        for (int kt = 0; kt < KT; ++kt) {
+          const int s = kt % TSTAGES, use = kt / TSTAGES, kb = kt0 + kt;
+          if (use > 0) mbar_wait(empty0 + 8 * s, (use - 1) & 1);
+          const uint32_t sw = sbase + s * STAGE_BYTES, sx = sw + W_BYTES;
+          mbar_expect_tx(full0 + 8 * s, ng * 1024 + X_BYTES);
+          const uint8_t* src = src0 + (int64_t)(kb >> 2) * MEGA_F8_TILE_BYTES + (kb & 3) * 1024;
+          for (int q = 0; q < ng; ++q) bulk_load(sw + q * 1024, src + q * gstride, 1024, full0 + 8 * s);
+          tma_load_2d(sx, &mapX, kb * TBK, 0, full0 + 8 * s);
+        }
+      } else {
+        for (int kt = 0; kt < KT; ++kt) {
+          const int s = kt % TSTAGES, use = kt / TSTAGES;
+          if (use > 0) mbar_wait(empty0 + 8 * s, (use - 1) & 1);
+          const uint32_t sw = sbase + s * STAGE_BYTES, sx = sw + A_BYTES;
+          mbar_expect_tx(full0 + 8 * s, STAGE_BYTES);
+          tma_load_2d(sw, &mapW, (kt0 + kt) * TBK, n0, full0 + 8 * s);
+          tma_load_2d(sx, &mapX, (kt0 + kt) * TBK, 0, full0 + 8 * s);
+        }
       }
     }
   } else {
@@ -271,16 +298,52 @@ __global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_
     float acc[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    float s0 = 0.f, s1 = 0.f;   // F8: row scales 2^k_r of this thread's rows g and g + 8
+    if constexpr (F8) {
+      const int gi = n0 / 16 + warp;
+      if (gi < f8.groups) { s0 = pow2f(f8.exps[gi * 16 + g]); s1 = pow2f(f8.exps[gi * 16 + g + 8]); }
+    }
     for (int kt = 0; kt < KT; ++kt) {
       const int s = kt % TSTAGES, use = kt / TSTAGES;
       mbar_wait(full0 + 8 * s, use & 1);
-      const uint32_t sw = sbase + s * STAGE_BYTES + wg * (64 * 128), sx = sbase + s * STAGE_BYTES + A_BYTES;
-      wgmma_acc_fence(acc);
-      wgmma_fence();
+      if constexpr (F8) {
+        const uint32_t sw = sbase + s * STAGE_BYTES + warp * 1024 + lane * 16, sx = sbase + s * STAGE_BYTES + W_BYTES;
+        uint4 q[2];
 #pragma unroll
-      for (int k = 0; k < TBK / 16; ++k) wgmma_tile(acc, wgmma_desc(sw + k * 32), wgmma_desc(sx + k * 32), (kt | k) != 0);
+        for (int h = 0; h < 2; ++h)
+          asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[h].x), "=r"(q[h].y), "=r"(q[h].z), "=r"(q[h].w) : "r"(sw + h * 512));
+        // k-step 2 h + u: word 2 u = fragments 0 | 1 (rows g | g + 8, k 2c), word 2 u + 1 = fragments 2 | 3 (k 8 + 2c)
+        // A operands are read asynchronously: the previous k-block's wgmma must be done with its registers before they are
+        // rebuilt (the bf16 tile keeps one k-block in flight; here it overlaps only the wait and the shared loads)
+        if (kt > 0) {
+          wgmma_wait<0>();
+          if (lane == 0) mbar_arrive(empty0 + 8 * ((kt - 1) % TSTAGES));
+        }
+        uint32_t a[4][4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t w[4] = {q[h].x, q[h].y, q[h].z, q[h].w};
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            a[2 * h + u][0] = e4m3x2_to_bf16x2(w[2 * u], s0);
+            a[2 * h + u][1] = e4m3x2_to_bf16x2(w[2 * u] >> 16, s1);
+            a[2 * h + u][2] = e4m3x2_to_bf16x2(w[2 * u + 1], s0);
+            a[2 * h + u][3] = e4m3x2_to_bf16x2(w[2 * u + 1] >> 16, s1);
+          }
+        }
+        wgmma_acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TBK / 16; ++k) wgmma_tile_rs(acc, a[k], wgmma_desc(sx + k * 32), (kt | k) != 0);
+      } else {
+        const uint32_t sw = sbase + s * STAGE_BYTES + wg * (64 * 128), sx = sbase + s * STAGE_BYTES + A_BYTES;
+        wgmma_acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TBK / 16; ++k) wgmma_tile(acc, wgmma_desc(sw + k * 32), wgmma_desc(sx + k * 32), (kt | k) != 0);
+      }
       wgmma_commit();
-      if (kt > 0) {
+      if (!F8 && kt > 0) {
         wgmma_wait<1>();
         if (lane == 0) mbar_arrive(empty0 + 8 * ((kt - 1) % TSTAGES));
       }
@@ -307,29 +370,62 @@ __global__ void __launch_bounds__(STHREADS, 2) gemm_tc_swap_kernel(const __grid_
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] += t[i];
       }
-      // rows = output features n (g and g + 8 of this warp's 16), columns = batch rows b
-      const int nA = n0 + wg * 64 + (warp & 3) * 16 + g;
+      if constexpr (F8) {
+        // rows g and g + 8 of group gi = output features tile_row(...): TILE_ROPE stores q / k / v in natural order, and in
+        // TILE_GLU they are (gate_i, up_i) of i = 8 gi + g, both in this thread (no shuffle)
+        const int gi = n0 / 16 + warp;
+        if (gi < f8.groups) {
+          const int nr[2] = {tile_row(f8.mode, f8.hd, gi, g), tile_row(f8.mode, f8.hd, gi, g + 8)};
 #pragma unroll
-      for (int i = 0; i < NACC; ++i) {
-        const int j = i >> 2, n = nA + ((i & 2) ? 8 : 0), b = 8 * j + 2 * c + (i & 1);
-        float v = acc[i];
-        if (p.bias && n < p.N) v += __bfloat162float(p.bias[n]);
-        if (p.glu) {
-          const float other = __shfl_xor_sync(0xffffffffu, v, 4);   // rows (gate, up) = lanes g, g + 1
-          if (!(g & 1) && n < p.N && b < p.M) {
-            const float rr = silu(v) * other;
-            const int64_t o = (int64_t)b * p.ldo + (n >> 1);
-            if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
-            else p.out_f32[o] = rr;
+          for (int i = 0; i < NACC; ++i)
+            if (p.bias && nr[(i >> 1) & 1] < p.N) acc[i] += __bfloat162float(p.bias[nr[(i >> 1) & 1]]);
+#pragma unroll
+          for (int i = 0; i < NACC; ++i) {
+            const int j = i >> 2, n = nr[(i >> 1) & 1], b = 8 * j + 2 * c + (i & 1);
+            float v = acc[i];
+            if (p.glu) {
+              if (!(i & 2) && n < p.N && b < p.M) {
+                const float rr = silu(v) * acc[i | 2];
+                const int64_t o = (int64_t)b * p.ldo + gi * 8 + g;
+                if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
+                else p.out_f32[o] = rr;
+              }
+              continue;
+            }
+            if (n < p.N && b < p.M) {
+              if (p.gate) v *= 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
+              if (p.resid) v += p.resid[(int64_t)b * p.ldr + n];
+              const int64_t o = (int64_t)b * p.ldo + n;
+              if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(v);
+              else p.out_f32[o] = v;
+            }
           }
-          continue;
         }
-        if (n < p.N && b < p.M) {
-          if (p.gate) v *= 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
-          if (p.resid) v += p.resid[(int64_t)b * p.ldr + n];
-          const int64_t o = (int64_t)b * p.ldo + n;
-          if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(v);
-          else p.out_f32[o] = v;
+      } else {
+        // rows = output features n (g and g + 8 of this warp's 16), columns = batch rows b
+        const int nA = n0 + wg * 64 + (warp & 3) * 16 + g;
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) {
+          const int j = i >> 2, n = nA + ((i & 2) ? 8 : 0), b = 8 * j + 2 * c + (i & 1);
+          float v = acc[i];
+          if (p.bias && n < p.N) v += __bfloat162float(p.bias[n]);
+          if (p.glu) {
+            const float other = __shfl_xor_sync(0xffffffffu, v, 4);   // rows (gate, up) = lanes g, g + 1
+            if (!(g & 1) && n < p.N && b < p.M) {
+              const float rr = silu(v) * other;
+              const int64_t o = (int64_t)b * p.ldo + (n >> 1);
+              if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(rr);
+              else p.out_f32[o] = rr;
+            }
+            continue;
+          }
+          if (n < p.N && b < p.M) {
+            if (p.gate) v *= 1.f / (1.f + expf(-__bfloat162float(*p.gate)));
+            if (p.resid) v += p.resid[(int64_t)b * p.ldr + n];
+            const int64_t o = (int64_t)b * p.ldo + n;
+            if (p.out_bf16) p.out_bf16[o] = __float2bfloat16_rn(v);
+            else p.out_f32[o] = v;
+          }
         }
       }
     }
@@ -408,17 +504,18 @@ static cudaError_t launch_tc_dense(const typename DenseArgs<LSE>::type& a, bool 
 static int g_swap_split = 0;   // dev switch (dtk_set_option "gemm_swap_split"): 0 = heuristic, 1..8 = forced split-K factor
 void set_gemm_swap_split(int v) { g_swap_split = v; }
 
-template <int NB, int TSTAGES>
-static cudaError_t launch_tc_swap(const GemmArgs& a, cudaStream_t s, uint64_t* counter) {
-  CUtensorMap mapW, mapX;
-  if (!make_map(&mapW, a.W, a.N, a.K, a.ldw, TBM) || !make_map(&mapX, a.A, a.M, a.K, a.lda, NB)) return cudaErrorInvalidValue;
-  constexpr int smem = TSTAGES * (A_BYTES + NB * TBK * 2) + 1024 + 256;
+// F8: the weights come from w (mapW is not used); the same grid and split-K factor as the bf16 tile of the same N and K
+template <int NB, int TSTAGES, bool F8 = false>
+static cudaError_t launch_tc_swap(const GemmArgs& a, cudaStream_t s, uint64_t* counter, const GemmF8& w = GemmF8{}) {
+  CUtensorMap mapW{}, mapX;
+  if ((!F8 && !make_map(&mapW, a.W, a.N, a.K, a.ldw, TBM)) || !make_map(&mapX, a.A, a.M, a.K, a.lda, NB)) return cudaErrorInvalidValue;
+  constexpr int smem = TSTAGES * ((F8 ? TBM * TBK : A_BYTES) + NB * TBK * 2) + 1024 + 256;
   static bool attr_done[64] = {};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   if (dev < 0 || dev >= 64 || !attr_done[dev]) {
-    e = cudaFuncSetAttribute(gemm_tc_swap_kernel<NB, TSTAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    e = cudaFuncSetAttribute(gemm_tc_swap_kernel<NB, TSTAGES, F8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
@@ -445,7 +542,7 @@ static cudaError_t launch_tc_swap(const GemmArgs& a, cudaStream_t s, uint64_t* c
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, gemm_tc_swap_kernel<NB, TSTAGES>, mapW, mapX, a, nsplit);
+  e = cudaLaunchKernelEx(&cfg, gemm_tc_swap_kernel<NB, TSTAGES, F8>, mapW, mapX, a, nsplit, w);
   if (counter) ++*counter;
   return e;
 }
@@ -459,6 +556,16 @@ cudaError_t launch_gemm_tc(const GemmArgs& a, cudaStream_t s, uint64_t* counter)
   // no such epilogue, so these few small products run on a 128-row tile that is mostly TMA zero fill
   if (get_gemm_impl() == 2) return launch_tc_dense<256>(a, true, s, counter);   // persistent 128 x 256
   return launch_tc_dense<128>(a, false, s, counter);
+}
+
+cudaError_t launch_gemm_swap_f8(const GemmArgs& a, const GemmF8& w, cudaStream_t s, uint64_t* counter) {
+  if (a.M <= 0 || a.N <= 0 || a.K <= 0) return cudaSuccess;
+  if (a.M >= 64 || a.act != ACT_NONE || a.rowbias || !w.tiles || !w.exps || (a.glu != 0) != (w.mode == TILE_GLU) ||
+      (int64_t)w.groups * 16 < a.N || (int64_t)w.tpg * 256 < a.K || !gemm_tc_supported(a))
+    return cudaErrorInvalidValue;
+  if (w.mode == TILE_ROPE && ((w.hd != 64 && w.hd != 128) || a.N % w.hd)) return cudaErrorInvalidValue;
+  // 9 / 6 stages: the deepest rings of 8 KB weight blocks that still fit two CTAs per SM
+  return a.M <= 32 ? launch_tc_swap<32, 9, true>(a, s, counter, w) : launch_tc_swap<64, 6, true>(a, s, counter, w);
 }
 
 cudaError_t launch_gemm_lse(const GemmLseArgs& a, cudaStream_t s, uint64_t* counter) {

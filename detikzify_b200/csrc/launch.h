@@ -53,6 +53,16 @@ cudaError_t launch_gemm_lse(const GemmLseArgs& a, cudaStream_t s, uint64_t* coun
 // logprob[m] = tgt[m] - lse[m] when targets[m] is in [0, N), else 0
 cudaError_t launch_lse_merge(const float2* part, const float* tgt, const int64_t* targets, int M, int N, float* logprob,
                              float* lse, cudaStream_t s, uint64_t* counter);
+// FP8 weight operand of the batched-decode GEMM: one layer matrix as decode tiles (launch_retile_f8, row order tile_row)
+struct GemmF8 {
+  const uint8_t* tiles;       // [groups][tpg] e4m3 tiles of MEGA_F8_TILE_BYTES
+  const int8_t* exps;         // [groups][16] row exponents k_r
+  int groups, tpg, mode, hd;  // MegaMat geometry and row permutation (hd: head_dim of TILE_ROPE)
+};
+// out = A W~^T on the swapped-operand wgmma tile (4 <= M < 64) with W~ = code x 2^k_r from the tiles: the same result bits as
+// launch_gemm on a bf16 W holding W~, with the same split-K cuts (N, K, glu and the epilogue fields as for launch_gemm;
+// W / ldw unused; glu requires TILE_GLU tiles). Other M, an activation or a row bias: cudaErrorInvalidValue.
+cudaError_t launch_gemm_swap_f8(const GemmArgs& a, const GemmF8& w, cudaStream_t s, uint64_t* counter);
 void set_gemm_swap_split(int v);    // dev: 0 (default) = heuristic split-K factor of the swapped tile, 1..8 = forced
 void set_gemm_impl(int impl);   // 0 = mma.sync everywhere, 1 = wgmma one 128 x 128 tile per CTA, 2 = persistent 128 x 256 wgmma (process-wide dev switch)
 int get_gemm_impl();

@@ -113,7 +113,8 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
 
     ``quantize="fp8"``: weight-only e4m3 quantization of the decoder-layer matrices (q/k/v/o, gate/up, down) with one
     power-of-two scale per output row (``detikzify_b200.quant``). The arena holds the dequantized values, so every path
-    computes the same quantized model, and batch-1 decode streams the layer matrices as e4m3 (about half the bytes).
+    computes the same quantized model, and batch-1 decode and batched decode steps of 4 <= B < 64 rows (rollouts,
+    ``generate_batch``) stream the layer matrices as e4m3 (about half the bytes) with bit-identical logits.
     Embeddings, norms, lm_head, projector, vision tower and KV cache stay bf16. ``None`` (default) keeps the weights as
     they are.
     """

@@ -5,7 +5,8 @@ Each output row ``r`` of a matrix ``W`` is stored as ``W~[r] = q[r] * 2^k_r``: `
 ``max |W[r]| <= 448 * 2^k_r`` (at least -117, so that every nonzero value stays a bf16 normal; 0 for a row of zeros) and
 ``q[r] = e4m3fn(W[r] / 2^k_r)`` rounded to nearest even. Because the scale is a power of two, ``W~`` is exactly
 representable in bf16: the quantized model is the bf16 model with ``W~`` in place of ``W``, on every path. The batch-1
-persistent decode kernel streams ``q`` and ``k_r`` instead of the bf16 values (engine option ``decode_fp8``).
+persistent decode kernel and the layer GEMMs of batched decode steps with 4 <= B < 64 rows stream ``q`` and ``k_r`` instead
+of the bf16 values (engine option ``decode_fp8``).
 """
 from __future__ import annotations
 

@@ -226,10 +226,11 @@ DTK_API int dtk_gen_end(dtk_engine* eng);
  *      mma.sync), "cascade_attn" (shared-prefix attention of batched decode), "decode_gemm_min_batch",
  *      "fuse_greedy", "vit_graph", and dev switches "mega_debug", "mega_flags", "mega_trace_layer",
  *      "mega_nslots", "mega_variant". Unknown keys return DTK_ERR_INVALID.
- *      "decode_fp8": 1 = the persistent kernel streams the four decoder-layer matrices as e4m3 codes plus one
- *      power-of-two exponent per row (rebuilt from the arena, whose every row must be e4m3 x 2^k; otherwise
- *      DTK_ERR_INVALID names the layer and matrix and nothing changes), 0 (default) = bf16 tiles. Its logits
- *      equal the bf16 kernel's on the same arena. ------------------------------------------------------ */
+ *      "decode_fp8": 1 = the persistent kernel (B = 1) and the four layer GEMMs of batched steps with
+ *      4 <= B < 64 stream the four decoder-layer matrices as e4m3 codes plus one power-of-two exponent per row
+ *      (rebuilt from the arena, whose every row must be e4m3 x 2^k; otherwise DTK_ERR_INVALID names the layer
+ *      and matrix and nothing changes), 0 (default) = bf16. The logits equal the bf16 kernels' on the same
+ *      arena; B = 2, 3, B >= 64 and the lm_head always run bf16. --------------------------------------- */
 DTK_API int dtk_set_option(dtk_engine* eng, const char* key, int64_t value);
 /*      Read back an option; the extra key "decode_persistent" reports whether B = 1 decode steps
  *      actually run on the persistent kernel (option set AND the device can co-schedule its grid), and
