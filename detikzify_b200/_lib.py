@@ -87,6 +87,7 @@ SYMBOLS = {
     "dtk_launch_count": (C.c_uint64, [_P]),
     "dtk_dbg_mega_times": (C.c_int, [_P, C.POINTER(C.c_longlong), C.c_int]),
     "dtk_dbg_mega_trace": (C.c_int, [_P, C.POINTER(C.c_longlong), C.c_int]),
+    "dtk_dbg_pack_bytes": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
     "dtk_dbg_gemm_impl": (C.c_int, [C.c_int]),
     "dtk_dbg_gemm": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "dtk_dbg_lm_logprob": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),

@@ -326,10 +326,13 @@ DTK_DEV float slices_rn(const float* slice_ss, int nslice, int K, float eps) {
 // then lm_head) with a single copy of the tile code and a run-time phase switch in the epilogue: the per-token
 // instruction footprint of a warp stays inside the SM's 32 KB instruction cache (the fully specialised version was
 // ~160 KB, re-fetched from L2 every layer: the first tiles of every phase ran 3-6x slower than the steady state).
-// F8 = true: the four layer matrices stream as e4m3 tiles (MegaF8); the consumers turn each A fragment into the bf16 bits
-// of code x 2^k_r and run the same mma sequence, so the logits equal those of the bf16 kernel on the dequantised weights.
-template <bool DBG, int HD, bool F8>
+// FMT = tile format of the weight stream. 0: bf16 tiles. 1 (F8): the four layer matrices stream as e4m3 tiles (MegaF8); the
+// consumers turn each A fragment into the bf16 bits of code x 2^k_r and run the same mma sequence, so the logits equal those of
+// the bf16 kernel on the dequantised weights. 2 (PK): every matrix, lm_head included, streams as packed tiles (MegaPack, 13
+// bits per weight); the consumers rebuild the exact bf16 bits of the A fragments in registers: the same logits as format 0.
+template <bool DBG, int HD, int FMT>
 __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const MegaArgs p) {
+  constexpr bool F8 = FMT == 1, PK = FMT == 2;
   constexpr int HALF = HD / 2;
   constexpr int LPK = HD / 8;                // attention: lanes per key (8 bf16 each)
   constexpr int NGRP = 32 / LPK;             // key groups per warp
@@ -462,6 +465,12 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
               if (evf) bulk_g2s_hint(dst, src, MEGA_F8_TILE_BYTES, fb, pol);
               else bulk_g2s(dst, src, MEGA_F8_TILE_BYTES, fb);
               bulk_g2s(dst + MEGA_F8_TILE_BYTES, f8.exps + (int64_t)l * f8.exp_stride + (int64_t)(g0 + (int)jk) * 16, 16, fb);
+            } else if (PK) {
+              const MegaPack& pk = p.pk[mat_of(ph)];
+              const uint8_t* src = pk.tiles + (int64_t)l * pk.layer_stride + ((int64_t)g0 * tpg + j) * MEGA_PK_TILE_BYTES;
+              mbar_expect_tx(fb, MEGA_PK_TILE_BYTES);
+              if (evf) bulk_g2s_hint(dst, src, MEGA_PK_TILE_BYTES, fb, pol);
+              else bulk_g2s(dst, src, MEGA_PK_TILE_BYTES, fb);
             } else {
               mbar_expect_tx(fb, TILE_BYTES);
               if (evf) bulk_g2s_hint(dst, base + (int64_t)j * MEGA_TILE_ELEMS, TILE_BYTES, fb, pol);
@@ -898,6 +907,83 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
             }
             rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);
             rA2 = (acc[2] + c1[2]) + (acc[3] + c1[3]);
+          } else if (PK) {
+            // ---- packed tile (MegaPack): one pair of an A fragment = two bytes sign | mantissa7 (word w of the byte plane, the
+            // same order as the e4m3 codes) and two exponent bytes (cb, the matching word of exponent codes, or of biased
+            // exponents in an escape tile): prmt spreads the bytes into the bf16 halves (the sign replicated up to bit 15),
+            // the codes go to bits 7..11 and the row base is added there. Rows g and g + 8 of the group: one base each.
+            cur_slot = sl;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
+            const uint32_t tb = ring_u32 + sl * TILE_BYTES;
+            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
+            uint4 q[8], nb[4], hb;
+            // the tile is read in two halves of 4 kstep pairs (bytes and codes), the slot handed back after the second: the first
+            // half's mma run while the second half is still in flight, and the A operands of 8 ksteps are live at a time
+            auto ld_half = [&](int h) {
+#pragma unroll
+              for (int s = 4 * h; s < 4 * h + 4; ++s)
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[s].x), "=r"(q[s].y), "=r"(q[s].z), "=r"(q[s].w) : "r"(tb + lane * 16 + s * 512));
+#pragma unroll
+              for (int s = 2 * h; s < 2 * h + 2; ++s)
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(nb[s].x), "=r"(nb[s].y), "=r"(nb[s].z), "=r"(nb[s].w) : "r"(tb + MEGA_PK_NIB + lane * 16 + s * 512));
+            };
+            ld_half(0);
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(hb.x), "=r"(hb.y), "=r"(hb.z), "=r"(hb.w) : "r"(tb + MEGA_PK_HB + lane * 16));
+            uint32_t r0, r1;
+            int ei;
+            asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r0) : "r"(tb + MEGA_PK_HDR + (lane >> 2)));
+            asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r1) : "r"(tb + MEGA_PK_HDR + 8 + (lane >> 2)));
+            asm volatile("ld.shared.s32 %0, [%1];\n" : "=r"(ei) : "r"(tb + MEGA_PK_HDR + 16));
+            // kstep pairs [4 h, 4 h + 4); cbw(s): the exponent bytes of the 16 values of kstep pair s, one word per word of q[s]
+            auto tile_mma = [&](int h, uint32_t bb0, uint32_t bb1, auto&& cbw) {
+#pragma unroll
+              for (int s = 4 * h; s < 4 * h + 4; ++s) {
+                const uint4 cb = cbw(s);
+                const uint32_t w[4] = {q[s].x, q[s].y, q[s].z, q[s].w}, e[4] = {cb.x, cb.y, cb.z, cb.w};
+                uint32_t a[2][4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                  uint32_t s0, s1;
+                  asm("prmt.b32 %0, %1, 0, 0x9180;\n" : "=r"(s0) : "r"(w[k]));
+                  asm("prmt.b32 %0, %1, 0, 0xB3A2;\n" : "=r"(s1) : "r"(w[k]));
+                  a[k >> 1][2 * (k & 1)] = (__byte_perm(e[k], 0u, 0x4140) << 7) + ((s0 & 0x807F807Fu) | bb0);
+                  a[k >> 1][2 * (k & 1) + 1] = (__byte_perm(e[k], 0u, 0x4342) << 7) + ((s1 & 0x807F807Fu) | bb1);
+                }
+                const uint2 b0 = xp[16 * s], b1 = xp[16 * s + 8];   // the input vector's B fragments of ksteps 2 s, 2 s + 1
+                mma_bf16_16816(acc, a[0], b0.x, b0.y);
+                mma_bf16_16816(c1, a[1], b1.x, b1.y);
+              }
+            };
+            // code of byte i of word k of kstep pair s: nibble i of nibble word k >> 1 (low / high half by k & 1), bit
+            // 8 i + 4 (s & 1) + k of high-bit word s >> 1; one lop3 merges them into a byte per value
+            auto codes = [&](int s) {
+              const uint32_t n0 = (s & 1) ? nb[s >> 1].z : nb[s >> 1].x, n1 = (s & 1) ? nb[s >> 1].w : nb[s >> 1].y;
+              const uint32_t hw = (s >> 1) == 0 ? hb.x : (s >> 1) == 1 ? hb.y : (s >> 1) == 2 ? hb.z : hb.w;
+              uint32_t cb[4];
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const int t = 4 * (s & 1) + k;   // the code's high bit goes from bit 8 i + t to bit 8 i + 4
+                const uint32_t hs = t >= 4 ? hw >> (t - 4) : hw << (4 - t);
+                cb[k] = (((k >> 1) ? n1 : n0) >> (4 * (k & 1)) & 0x0F0F0F0Fu) | (hs & 0x10101010u);
+              }
+              return make_uint4(cb[0], cb[1], cb[2], cb[3]);
+            };
+            // escape tile: the biased exponents themselves, from the side buffer (base 0)
+            const uint4* ep = reinterpret_cast<const uint4*>(p.pk_esc + (int64_t)(ei < 0 ? 0 : ei) * MEGA_PK_ESC_BYTES) + lane;
+            auto escaped = [&](int s) { return __ldg(ep + s * 32); };
+            const uint32_t bb0 = r0 * 0x00800080u, bb1 = r1 * 0x00800080u;   // row base at bits 7 and 23
+            if (!(dflags & 1)) {
+              if (ei < 0) tile_mma(0, bb0, bb1, codes);
+              else tile_mma(0, 0u, 0u, escaped);
+            }
+            ld_half(1);
+            release();
+            if (!(dflags & 1)) {
+              if (ei < 0) tile_mma(1, bb0, bb1, codes);
+              else tile_mma(1, 0u, 0u, escaped);
+            }
+            rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);
+            rA2 = (acc[2] + c1[2]) + (acc[3] + c1[3]);
           } else {
             cur_slot = sl;
             float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
@@ -1091,6 +1177,90 @@ __global__ void __launch_bounds__(256) f8_tile_kernel(const bf16* __restrict__ s
   *reinterpret_cast<uint4*>(dst + q * 16) = make_uint4(out[0], out[1], out[2], out[3]);
 }
 
+// Packed tiles, pass 1: one CTA per tile, warp w takes tile rows w and w + 8 (8 columns per lane). Row base b_r = max(row max
+// exponent - 31, 0) over the row's values inside the matrix; the tile escapes when a value's exponent lies below its row's base.
+__global__ void __launch_bounds__(256) pk_scan_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int tpg,
+                                                      uint8_t* __restrict__ dst, uint8_t* __restrict__ escape) {
+  const int64_t tile = blockIdx.x;
+  const int ks = (int)(tile % tpg), gi = (int)(tile / tpg);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t base[2];
+  bool esc = false;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = tile_row(mode, hd, gi, warp + 8 * h), col = ks * 256 + lane * 8;
+    uint32_t emax = 0, emin = 255;
+    if (row < N && col < K) {   // K % 8 == 0: the lane's 8 columns are all inside or all outside
+      const uint4 v = *reinterpret_cast<const uint4*>(src + (int64_t)row * K + col);
+      const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t e0 = (u[i] >> 7) & 0xffu, e1 = (u[i] >> 23) & 0xffu;
+        emax = max(emax, max(e0, e1));
+        emin = min(emin, min(e0, e1));
+      }
+    }
+    emax = __reduce_max_sync(0xffffffffu, emax);
+    emin = __reduce_min_sync(0xffffffffu, emin);
+    base[h] = emax > 31u ? emax - 31u : 0u;
+    esc = esc || emin < base[h];
+  }
+  esc = __syncthreads_or(esc) != 0;
+  uint8_t* hdr = dst + tile * MEGA_PK_TILE_BYTES + MEGA_PK_HDR;
+  if (lane == 0) {
+    hdr[warp] = esc ? 0 : (uint8_t)base[0];
+    hdr[warp + 8] = esc ? 0 : (uint8_t)base[1];
+  }
+  if (threadIdx.x == 0) escape[tile] = esc ? 1 : 0;
+}
+
+// Packed tiles, pass 2: one thread per (tile, lane) writes the lane's bytes of every plane (value order of f8_tile_kernel)
+__global__ void __launch_bounds__(256) pk_tile_kernel(const bf16* __restrict__ src, int N, int K, int mode, int hd, int groups,
+                                                      int tpg, const int* __restrict__ esc_idx, uint8_t* __restrict__ dst,
+                                                      uint8_t* __restrict__ esc) {
+  const int64_t q = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (q >= (int64_t)groups * tpg * 32) return;
+  const int lane = (int)(q & 31);
+  const int64_t tile = q >> 5;
+  const int ks = (int)(tile % tpg), gi = (int)(tile / tpg);
+  uint8_t* t = dst + tile * MEGA_PK_TILE_BYTES;
+  const int ei = esc_idx[tile];
+  const uint32_t rb[2] = {t[MEGA_PK_HDR + (lane >> 2)], t[MEGA_PK_HDR + 8 + (lane >> 2)]};
+  uint32_t hbw[4] = {0u, 0u, 0u, 0u};
+  for (int p = 0; p < 8; ++p) {
+    uint32_t bytes[4], ex[4], nib[2] = {0u, 0u};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {   // word k: kstep 2p + (k >> 1), fragments 2 (k & 1) and 2 (k & 1) + 1 (bytes 0-1 / 2-3)
+      uint32_t bw = 0, xw = 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int m = 2 * (k & 1) + (i >> 1);   // fragment: rows-half m & 1, k-half m >> 1
+        const int ar = (m & 1) * 8 + (lane >> 2);
+        const int row = tile_row(mode, hd, gi, ar);
+        const int col = ks * 256 + (2 * p + (k >> 1)) * 16 + (m >> 1) * 8 + 2 * (lane & 3) + (i & 1);
+        const bool in = row < N && col < K;
+        const uint32_t v = in ? (uint32_t)__bfloat16_as_ushort(src[(int64_t)row * K + col]) : 0u;
+        const uint32_t e = (v >> 7) & 0xffu;
+        bw |= (((v >> 8) & 0x80u) | (v & 0x7fu)) << (8 * i);
+        xw |= e << (8 * i);
+        if (ei < 0) {
+          const uint32_t c = in ? e - rb[m & 1] : 0u;   // 0..31 outside an escape tile (pass 1)
+          nib[k >> 1] |= (c & 15u) << (8 * i + 4 * (k & 1));
+          hbw[p >> 1] |= (c >> 4) << (8 * i + 4 * (p & 1) + k);
+        }
+      }
+      bytes[k] = bw;
+      ex[k] = xw;
+    }
+    *reinterpret_cast<uint4*>(t + p * 512 + lane * 16) = make_uint4(bytes[0], bytes[1], bytes[2], bytes[3]);
+    *reinterpret_cast<uint2*>(t + MEGA_PK_NIB + (p >> 1) * 512 + lane * 16 + (p & 1) * 8) = make_uint2(nib[0], nib[1]);
+    if (ei >= 0)
+      *reinterpret_cast<uint4*>(esc + (int64_t)ei * MEGA_PK_ESC_BYTES + p * 512 + lane * 16) = make_uint4(ex[0], ex[1], ex[2], ex[3]);
+  }
+  *reinterpret_cast<uint4*>(t + MEGA_PK_HB + lane * 16) = make_uint4(hbw[0], hbw[1], hbw[2], hbw[3]);
+  if (lane == 0) *reinterpret_cast<uint4*>(t + MEGA_PK_HDR + 16) = make_uint4((uint32_t)ei, 0u, 0u, 0u);
+}
+
 }  // namespace
 
 int64_t mega_tiled_elems(int N, int K, int mode, int* groups, int* tpg) {
@@ -1118,6 +1288,24 @@ cudaError_t launch_retile_f8(const bf16* src, int N, int K, int mode, int hd, ui
   f8_rows_kernel<<<(unsigned)((groups * 16 + 7) / 8), 256, 0, s>>>(src, N, K, mode, hd, groups, exps, bad);
   const int64_t chunks = (int64_t)groups * tpg * 256;
   f8_tile_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, s>>>(src, N, K, mode, hd, groups, tpg, exps, dst);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pack_scan(const bf16* src, int N, int K, int mode, int hd, uint8_t* dst, uint8_t* escape, cudaStream_t s) {
+  if ((K & 7) || (mode == TILE_ROPE && ((hd != 64 && hd != 128) || N % hd))) return cudaErrorInvalidValue;
+  int groups, tpg;
+  mega_tiled_elems(N, K, mode, &groups, &tpg);
+  pk_scan_kernel<<<(unsigned)(groups * tpg), 256, 0, s>>>(src, N, K, mode, hd, tpg, dst, escape);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pack_tiles(const bf16* src, int N, int K, int mode, int hd, const int* esc_idx, uint8_t* dst, uint8_t* esc,
+                              cudaStream_t s) {
+  if ((K & 7) || (mode == TILE_ROPE && ((hd != 64 && hd != 128) || N % hd))) return cudaErrorInvalidValue;
+  int groups, tpg;
+  mega_tiled_elems(N, K, mode, &groups, &tpg);
+  const int64_t threads = (int64_t)groups * tpg * 32;
+  pk_tile_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(src, N, K, mode, hd, groups, tpg, esc_idx, dst, esc);
   return cudaGetLastError();
 }
 
@@ -1159,12 +1347,12 @@ cudaError_t launch_decode_mega(const MegaArgs& a, int grid, cudaStream_t s, uint
   const int smem = mega_smem_bytes(a);
   const bool dbgk = a.dbg != nullptr || a.dbg2 != nullptr || a.dbg_flags != 0;
   const void* fn;
-  const bool f8 = a.f8[0].tiles != nullptr;
-  if (a.hd == 128 && !f8) fn = dbgk ? (const void*)decode_mega_kernel<true, 128, false> : (const void*)decode_mega_kernel<false, 128, false>;
-  else if (a.hd == 64 && !f8) fn = dbgk ? (const void*)decode_mega_kernel<true, 64, false> : (const void*)decode_mega_kernel<false, 64, false>;
-  else if (a.hd == 128) fn = dbgk ? (const void*)decode_mega_kernel<true, 128, true> : (const void*)decode_mega_kernel<false, 128, true>;
-  else if (a.hd == 64) fn = dbgk ? (const void*)decode_mega_kernel<true, 64, true> : (const void*)decode_mega_kernel<false, 64, true>;
+  const int fmt = a.pk[0].tiles ? 2 : a.f8[0].tiles ? 1 : 0;
+#define DTK_MEGA_FN(hd, f) (dbgk ? (const void*)decode_mega_kernel<true, hd, f> : (const void*)decode_mega_kernel<false, hd, f>)
+  if (a.hd == 128) fn = fmt == 0 ? DTK_MEGA_FN(128, 0) : fmt == 1 ? DTK_MEGA_FN(128, 1) : DTK_MEGA_FN(128, 2);
+  else if (a.hd == 64) fn = fmt == 0 ? DTK_MEGA_FN(64, 0) : fmt == 1 ? DTK_MEGA_FN(64, 1) : DTK_MEGA_FN(64, 2);
   else return cudaErrorInvalidValue;
+#undef DTK_MEGA_FN
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
   void* args[] = {(void*)&a};

@@ -252,6 +252,10 @@ struct dtk_engine {
   bf16* d_tiled_lm = nullptr;          // ... and of the lm_head (always bf16)
   uint8_t* d_tiled8 = nullptr;         // FP8 mode (option "decode_fp8"): e4m3 tiles, row exponents and check counters
   int decode_fp8 = 0;
+  uint8_t* d_tiledpk = nullptr;        // packed mode (option "decode_pack"): packed tiles of the layer matrices and the lm_head
+  uint8_t* d_pk_esc = nullptr;         // ... and the exponent planes of the escape tiles
+  int decode_pack = 0;
+  int64_t pk_escapes = 0;              // escape tiles of the packed weights
   unsigned long long* d_tagged = nullptr;  // {fp32 value, phase tag} cross-CTA activation words of the persistent kernel
   long long* d_dbg = nullptr;           // phase timestamps of the persistent kernel (option mega_debug)
   long long* d_dbg2 = nullptr;          // per-tile clock trace of one layer (option mega_trace_layer)
@@ -558,8 +562,34 @@ bf16* kv_layer(dtk_engine* eng, int slot, int layer) {
 }
 
 // Decode-side tiles of the four layer matrices from the arena: bf16 (MegaMat::base) or FP8 (MegaArgs::f8, which requires
-// every row of every layer matrix to be e4m3 x 2^k_r). The new tiles are built and checked in a buffer of their own; only
-// then are they swapped in and the other format's tiles freed, so a failure leaves the engine as it was.
+// every row of every layer matrix to be e4m3 x 2^k_r); the lm_head streams as bf16 tiles in both formats (d_tiled_lm, rebuilt
+// here after packed mode). The new tiles are built and checked in a buffer of their own; only then are they swapped in and the
+// other format's tiles freed, so a failure leaves the engine as it was.
+// Frees the decode tiles of the current format (the lm_head's bf16 tiles only in packed mode, where they are not read). Every
+// captured graph that bakes in MegaArgs or the FP8 tile pointers goes with them: the batched decode steps and the per-token
+// graph of a generation loop (which lives in the same cache).
+void drop_decode_tiles(dtk_engine* eng) {
+  for (auto& g : eng->graphs) cudaGraphExecDestroy(g.second);
+  eng->graphs.clear();
+  eng->gen_graph = nullptr;
+  cudaFree(eng->d_tiled);
+  cudaFree(eng->d_tiled8);
+  cudaFree(eng->d_tiledpk);
+  cudaFree(eng->d_pk_esc);
+  for (int i = 0; i < 4; ++i) eng->mega.mat[i].base = nullptr;
+  eng->d_tiled = nullptr;
+  eng->d_tiled8 = nullptr;
+  eng->d_tiledpk = eng->d_pk_esc = nullptr;
+  MegaArgs& m = eng->mega;
+  for (int i = 0; i < 5; ++i) m.pk[i] = MegaPack{};
+  for (int i = 0; i < 4; ++i) m.f8[i] = MegaF8{};
+  m.pk_esc = nullptr;
+  eng->decode_fp8 = eng->decode_pack = 0;
+  eng->pk_escapes = 0;
+}
+
+int mega_pack_tiles(dtk_engine* eng);
+
 int mega_layer_tiles(dtk_engine* eng, bool fp8) {
   static const char* names[4] = {"wqkv", "wo", "wgu", "wd"};
   const dtk_config& c = eng->cfg;
@@ -580,6 +610,11 @@ int mega_layer_tiles(dtk_engine* eng, bool fp8) {
   DTK_ALLOC(buf, total);
   unsigned int* bad = reinterpret_cast<unsigned int*>(buf + bad0);
   cudaError_t e = fp8 ? cudaMemset(bad, 0, 4 * (size_t)L * sizeof(unsigned int)) : cudaSuccess;
+  bf16* lm = nullptr;
+  if (e == cudaSuccess && !eng->d_tiled_lm) {
+    e = cudaMalloc(&lm, (size_t)m.mat[4].groups * m.mat[4].tpg * MEGA_TILE_ELEMS * sizeof(bf16));
+    if (e == cudaSuccess) e = launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, hd, lm, 0);
+  }
   for (int l = 0; l < L && e == cudaSuccess; ++l)
     for (int i = 0; i < 4 && e == cudaSuccess; ++i) {
       const MegaMat& mm = m.mat[i];
@@ -594,22 +629,20 @@ int mega_layer_tiles(dtk_engine* eng, bool fp8) {
   if (e == cudaSuccess && fp8) e = cudaMemcpy(nbad.data(), bad, nbad.size() * sizeof(unsigned int), cudaMemcpyDeviceToHost);
   if (e != cudaSuccess) {
     cudaFree(buf);
+    cudaFree(lm);
     eng->err = std::string("decode tiles: ") + cudaGetErrorString(e);
     return DTK_ERR_CUDA;
   }
   for (size_t k = 0; k < nbad.size(); ++k)
     if (nbad[k]) {
       cudaFree(buf);
+      cudaFree(lm);
       eng->err = "invalid argument: decode_fp8: layer " + std::to_string(k / 4) + " " + names[k % 4] + " holds " +
                  std::to_string(nbad[k]) + " values that are not an e4m3 value times a power-of-two row scale (quantize the "
                  "weights first: load(..., quantize=\"fp8\"))";
       return DTK_ERR_INVALID;
     }
-  // captured batched decode steps bake in the tile pointers of the old format, which are freed here
-  for (auto& g : eng->graphs) cudaGraphExecDestroy(g.second);
-  eng->graphs.clear();
-  cudaFree(eng->d_tiled);
-  cudaFree(eng->d_tiled8);
+  drop_decode_tiles(eng);
   eng->d_tiled = fp8 ? nullptr : reinterpret_cast<bf16*>(buf);
   eng->d_tiled8 = fp8 ? buf : nullptr;
   for (int i = 0; i < 4; ++i) {
@@ -617,17 +650,108 @@ int mega_layer_tiles(dtk_engine* eng, bool fp8) {
     m.mat[i].layer_stride = fp8 ? 0 : per_layer / 2;
     m.f8[i] = fp8 ? MegaF8{buf + off[i], reinterpret_cast<const int8_t*>(buf + exp0 + eoff[i]), per_layer, exp_layer} : MegaF8{};
   }
+  if (lm) eng->d_tiled_lm = lm;
+  m.mat[4].base = eng->d_tiled_lm;
   eng->decode_fp8 = fp8 ? 1 : 0;
+  return DTK_OK;
+}
+
+// Packed decode tiles (MegaArgs::pk) of the four layer matrices and the lm_head from the arena: lossless, any bf16 weights.
+// Two passes over every matrix: the first derives the row bases and marks the escape tiles, the host numbers the escape tiles
+// in tile order (deterministic side-buffer layout), the second writes the planes. Built in buffers of their own and swapped in
+// on success, as mega_layer_tiles.
+int mega_pack_tiles(dtk_engine* eng) {
+  static const char* names[4] = {"wqkv", "wo", "wgu", "wd"};
+  const dtk_config& c = eng->cfg;
+  MegaArgs& m = eng->mega;
+  const int hd = c.head_dim, L = c.layers;
+  int64_t per_layer = 0, toff[4];   // tiles
+  for (int i = 0; i < 4; ++i) {
+    toff[i] = per_layer;
+    per_layer += (int64_t)m.mat[i].groups * m.mat[i].tpg;
+  }
+  const int64_t lm0 = per_layer * L, ntiles = lm0 + (int64_t)m.mat[4].groups * m.mat[4].tpg;
+  DTK_CK(cudaDeviceSynchronize());   // the arena is written; no launch reads the current tiles any more
+  uint8_t *buf = nullptr, *flags = nullptr, *esc = nullptr;
+  int* idx = nullptr;
+  cudaError_t e = cudaMalloc(&buf, (size_t)ntiles * MEGA_PK_TILE_BYTES);
+  bool dropped = false;
+  if (e == cudaErrorMemoryAllocation) {
+    // no room for both tile sets (a 7B model with a large KV cache): the current tiles go first, and bf16 tiles are rebuilt
+    // from the arena if packing fails below
+    cudaGetLastError();
+    drop_decode_tiles(eng);
+    cudaFree(eng->d_tiled_lm);
+    eng->d_tiled_lm = nullptr;
+    dropped = true;
+    e = cudaMalloc(&buf, (size_t)ntiles * MEGA_PK_TILE_BYTES);
+  }
+  if (e == cudaSuccess) e = cudaMalloc(&flags, (size_t)ntiles);
+  if (e == cudaSuccess) e = cudaMalloc(&idx, (size_t)ntiles * sizeof(int));
+  // every matrix with the index of its first tile
+  auto each = [&](auto&& f) {
+    for (int l = 0; l < L && e == cudaSuccess; ++l)
+      for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = f(W(eng, LN("dec.L", l, names[i])), m.mat[i], l * per_layer + toff[i]);
+    if (e == cudaSuccess) e = f(W(eng, "dec.lm_head"), m.mat[4], lm0);
+  };
+  each([&](const bf16* src, const MegaMat& mm, int64_t t0) {
+    return launch_pack_scan(src, mm.N, mm.K, mm.mode, hd, buf + t0 * MEGA_PK_TILE_BYTES, flags + t0, 0);
+  });
+  std::vector<uint8_t> hflag(e == cudaSuccess ? ntiles : 0);
+  std::vector<int> hidx(hflag.size());
+  if (e == cudaSuccess) e = cudaMemcpy(hflag.data(), flags, hflag.size(), cudaMemcpyDeviceToHost);
+  int64_t nesc = 0;
+  for (size_t t = 0; t < hflag.size(); ++t) hidx[t] = hflag[t] ? (int)nesc++ : -1;
+  if (e == cudaSuccess) e = cudaMemcpy(idx, hidx.data(), hidx.size() * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && nesc) e = cudaMalloc(&esc, (size_t)nesc * MEGA_PK_ESC_BYTES);
+  each([&](const bf16* src, const MegaMat& mm, int64_t t0) {
+    return launch_pack_tiles(src, mm.N, mm.K, mm.mode, hd, idx + t0, buf + t0 * MEGA_PK_TILE_BYTES, esc, 0);
+  });
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  cudaFree(flags);
+  cudaFree(idx);
+  if (e != cudaSuccess) {
+    cudaFree(buf);
+    cudaFree(esc);
+    cudaGetLastError();
+    const std::string msg = std::string("packed decode tiles: ") + cudaGetErrorString(e);
+    if (dropped && mega_layer_tiles(eng, false) != DTK_OK) eng->err = msg + "; rebuilding the bf16 tiles failed: " + eng->err;
+    else eng->err = msg + (dropped ? " (the engine is back on bf16 tiles)" : "");
+    return DTK_ERR_CUDA;
+  }
+  drop_decode_tiles(eng);
+  cudaFree(eng->d_tiled_lm);
+  eng->d_tiled_lm = nullptr;
+  eng->d_tiledpk = buf;
+  eng->d_pk_esc = esc;
+  for (int i = 0; i < 5; ++i) {
+    m.mat[i].base = nullptr;
+    m.mat[i].layer_stride = 0;
+    m.pk[i] = MegaPack{buf + (i < 4 ? toff[i] : lm0) * MEGA_PK_TILE_BYTES, i < 4 ? per_layer * MEGA_PK_TILE_BYTES : 0};
+  }
+  m.pk_esc = esc;
+  eng->decode_pack = 1;
+  eng->pk_escapes = nesc;
   return DTK_OK;
 }
 
 // weight bytes one batch-1 persistent decode token streams: the four layer matrices (bf16, or e4m3 codes plus one exponent
 // per row), the lm_head in bf16
+// (packed mode: decode_pack_weight_bytes)
 uint64_t decode_weight_bytes(const dtk_config& c, bool fp8) {
   const uint64_t H = c.hidden, I = c.inter, V = c.vocab, qd = (uint64_t)c.heads * c.head_dim, kd = (uint64_t)c.kv_heads * c.head_dim;
   const uint64_t layer_w = (uint64_t)c.layers * ((qd + 2 * kd) * H + H * qd + 3 * H * I);
   const uint64_t layer_rows = (uint64_t)c.layers * ((qd + 2 * kd) + H + 2 * I + H);
   return (fp8 ? layer_w + layer_rows : 2 * layer_w) + 2 * V * H;
+}
+
+// packed mode: every tile of the layer matrices and the lm_head (planes and header) plus the escape tiles' exponent planes
+uint64_t decode_pack_weight_bytes(const dtk_engine* eng) {
+  const MegaArgs& m = eng->mega;
+  uint64_t layer = 0;
+  for (int i = 0; i < 4; ++i) layer += (uint64_t)m.mat[i].groups * m.mat[i].tpg;
+  const uint64_t tiles = layer * eng->cfg.layers + (uint64_t)m.mat[4].groups * m.mat[4].tpg;
+  return tiles * MEGA_PK_TILE_BYTES + (uint64_t)eng->pk_escapes * MEGA_PK_ESC_BYTES;
 }
 
 int nsplit_for(const dtk_config& c, int B) {
@@ -919,18 +1043,16 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
         mega_tiled_elems(specs[i].N, specs[i].K, specs[i].mode, &mm.groups, &mm.tpg);
         mm.N = specs[i].N; mm.K = specs[i].K; mm.mode = specs[i].mode;
       }
-      const int64_t lm_elems = mega_tiled_elems(c.vocab, c.hidden, TILE_SEQ, &m.mat[4].groups, &m.mat[4].tpg);
+      mega_tiled_elems(c.vocab, c.hidden, TILE_SEQ, &m.mat[4].groups, &m.mat[4].tpg);
+      m.mat[4].layer_stride = 0; m.mat[4].N = c.vocab; m.mat[4].K = c.hidden; m.mat[4].mode = TILE_SEQ;
       for (int i = 0; i < 5; ++i) {
         m.mat[i].per = (m.mat[i].groups + grid - 1) / grid;
         m.mat[i].nact = (m.mat[i].groups + m.mat[i].per - 1) / m.mat[i].per;
       }
       {
-        const int r = mega_layer_tiles(eng, false);
+        const int r = mega_layer_tiles(eng, false);   // bf16 tiles (and the lm_head's)
         if (r != DTK_OK) return r;
       }
-      DTK_ALLOC(eng->d_tiled_lm, lm_elems);
-      m.mat[4].base = eng->d_tiled_lm; m.mat[4].layer_stride = 0; m.mat[4].N = c.vocab; m.mat[4].K = c.hidden; m.mat[4].mode = TILE_SEQ;
-      DTK_CK(launch_retile(W(eng, "dec.lm_head"), c.vocab, c.hidden, TILE_SEQ, c.head_dim, eng->d_tiled_lm, 0));
       m.tok = eng->d_tok; m.pos = eng->d_pos; m.slots = eng->d_slots; m.share_slot = eng->d_share_slot; m.share_len = eng->d_share_len;
       m.kv = eng->kv; m.kv_slot_stride = eng->kv_slot_stride; m.kv_layer_stride = eng->kv_layer_stride;
       m.kv_v_offset = eng->kv_v_offset; m.rope_cs = eng->rope_cs;
@@ -973,7 +1095,7 @@ int dtk_destroy(dtk_engine* eng) {
   for (auto& g : eng->vit_graphs) cudaGraphExecDestroy(g.second.exec);
   void* ptrs[] = {eng->v_pix_in, eng->v_tok_out, eng->v_pool_out, eng->v_vt, eng->kv, eng->rope_cs, eng->p_x, eng->p_qkv, eng->p_xn, eng->p_q, eng->p_att, eng->p_h, eng->d_x, eng->d_q,
                   eng->d_att, eng->d_h, eng->d_logits, eng->d_scratch, eng->d_part_o, eng->d_part_ml, eng->d_counters,
-                  eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tiled_lm, eng->d_tiled8, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
+                  eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tiled_lm, eng->d_tiled8, eng->d_tiledpk, eng->d_pk_esc, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
                   eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt};
   for (void* p : ptrs) if (p) cudaFree(p);
   dtk_adapter_detach(eng);
@@ -1686,6 +1808,12 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
     if ((int)value == eng->decode_fp8) return DTK_OK;
     return mega_layer_tiles(eng, value == 1);
   }
+  if (std::strcmp(key, "decode_pack") == 0) {  // batch-1 persistent decode streams every matrix as packed 13-bit (1) or bf16 (0) tiles
+    DTK_REQUIRE(value == 0 || value == 1, "decode_pack must be 0 or 1");
+    DTK_REQUIRE(eng->mega_ok, "decode_pack: the persistent decode kernel is unavailable on this device");
+    if ((int)value == eng->decode_pack) return DTK_OK;
+    return value == 1 ? mega_pack_tiles(eng) : mega_layer_tiles(eng, false);
+  }
   if (std::strcmp(key, "mega_nslots") == 0) {  // dev: smaller ring (8 / 16) for A/B runs of the stream's depth
     eng->mega_nslots = (int)value;
     return DTK_OK;
@@ -1709,7 +1837,12 @@ int dtk_get_option(dtk_engine* eng, const char* key, int64_t* value) {
   if (std::strcmp(key, "mega_debug") == 0) { *value = eng->mega_debug; return DTK_OK; }
   if (std::strcmp(key, "mega_variant") == 0) { *value = eng->mega_variant; return DTK_OK; }
   if (std::strcmp(key, "decode_fp8") == 0) { *value = eng->decode_fp8; return DTK_OK; }
-  if (std::strcmp(key, "decode_weight_bytes") == 0) { *value = (int64_t)decode_weight_bytes(eng->cfg, eng->decode_fp8 != 0); return DTK_OK; }
+  if (std::strcmp(key, "decode_pack") == 0) { *value = eng->decode_pack; return DTK_OK; }
+  if (std::strcmp(key, "decode_pack_escapes") == 0) { *value = eng->pk_escapes; return DTK_OK; }
+  if (std::strcmp(key, "decode_weight_bytes") == 0) {
+    *value = (int64_t)(eng->decode_pack ? decode_pack_weight_bytes(eng) : decode_weight_bytes(eng->cfg, eng->decode_fp8 != 0));
+    return DTK_OK;
+  }
   eng->err = std::string("unknown option ") + key;
   return DTK_ERR_INVALID;
 }
@@ -1733,6 +1866,17 @@ int dtk_dbg_mega_trace(dtk_engine* eng, long long* out_host, int max_values) {
   DTK_CK(cudaDeviceSynchronize());
   DTK_CK(cudaMemcpy(out_host, eng->d_dbg2, (size_t)(n < max_values ? n : max_values) * sizeof(long long), cudaMemcpyDeviceToHost));
   return n;
+}
+
+int dtk_dbg_pack_bytes(dtk_engine* eng, int64_t offset, int64_t nbytes, void* out_host) {
+  if (!eng || !out_host) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->d_tiledpk != nullptr, "decode_pack is off");
+  const int64_t total = (int64_t)(decode_pack_weight_bytes(eng) - (uint64_t)eng->pk_escapes * MEGA_PK_ESC_BYTES);
+  DTK_REQUIRE(offset >= 0 && nbytes >= 0 && offset + nbytes <= total, "byte range outside the packed tiles");
+  DTK_CK(cudaSetDevice(eng->device));
+  DTK_CK(cudaDeviceSynchronize());
+  DTK_CK(cudaMemcpy(out_host, eng->d_tiledpk + offset, (size_t)nbytes, cudaMemcpyDeviceToHost));
+  return DTK_OK;
 }
 
 int dtk_dbg_gemm_impl(int impl) {

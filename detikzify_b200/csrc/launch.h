@@ -250,6 +250,23 @@ struct MegaF8 {
   int64_t layer_stride;   // bytes between layers of tiles
   int64_t exp_stride;     // bytes between layers of exps
 };
+// Packed decode tiles (launch_pack_scan / launch_pack_tiles): the same bf16 bits in 13 bits per weight, lossless. A tile of
+// 16 rows x 256 k is one 6688-byte block:
+//   [0, 4096)     sign | mantissa7 of each value, in the FP8 tile's order ([kstep pair 8][lane 32][16 B]);
+//   [4096, 6144)  low 4 bits of the exponent codes, [load 4][lane 32][16 B]: load i holds kstep pairs 2i and 2i + 1, 8 B each
+//                 (word w of a pair: byte i of words 2w and 2w + 1 of the pair's 16 bytes in its low / high nibble);
+//   [6144, 6656)  high bits of the codes, [lane 32][4 words]: word j = kstep pairs 2j, 2j + 1, bit 8 i + 4 (pair & 1) + word;
+//   [6656, 6688)  header: the exponent base b_r of each of the 16 tile rows, then the tile's escape entry (int32, -1 if none).
+// A value's biased exponent is b_r + code, b_r = max(row max exponent in the tile - 31, 0). A tile in which some value does not
+// fit (more than 31 binades below its row's largest value; also a zero or subnormal in a row with b_r > 0) is an ESCAPE tile:
+// its codes are zero, b_r = 0, and its full exponent bytes ([kstep pair][lane][16 B], 4096 B) live in a side buffer at entry
+// escape * 4096. The K padding of a tile decodes to a finite value that multiplies a zero input.
+constexpr int MEGA_PK_TILE_BYTES = 6688;
+constexpr int MEGA_PK_NIB = 4096, MEGA_PK_HB = 6144, MEGA_PK_HDR = 6656, MEGA_PK_ESC_BYTES = 4096;
+struct MegaPack {
+  const uint8_t* tiles;   // layer 0
+  int64_t layer_stride;   // bytes between layers
+};
 struct MegaArgs {
   int H, I, L, heads, kv_heads, V, max_len;
   int hd;                                                     // decoder head_dim, 64 or 128 (mega_configure)
@@ -283,6 +300,10 @@ struct MegaArgs {
   int dbg_layer;
   // FP8 decoder weights (option "decode_fp8"; null tiles = bf16): e4m3 tiles of the four layer matrices, same order as mat[0..3]
   MegaF8 f8[4];
+  // packed decoder weights (option "decode_pack"; null tiles = off): tiles of the four layer matrices and the lm_head, same order
+  // as mat[0..4], and the escape tiles' exponent planes
+  MegaPack pk[5];
+  const uint8_t* pk_esc;
 };
 int mega_smem_bytes(const MegaArgs& a);
 cudaError_t mega_configure(MegaArgs& a, int H, int I, int heads, int hd, int max_smem_optin, int num_sms, int* grid_out);
@@ -294,6 +315,12 @@ cudaError_t launch_retile(const bf16* src, int N, int K, int mode, int hd, bf16*
 // row of zeros) into exps and adds to *bad the number of values that are not an e4m3 value times 2^k_r (those tiles are junk)
 cudaError_t launch_retile_f8(const bf16* src, int N, int K, int mode, int hd, uint8_t* dst, int8_t* exps, unsigned int* bad,
                              cudaStream_t s);
+// the same matrix into packed tiles, in two passes. Scan: writes each tile's row bases into its header and escape[tile] = 1 for
+// an escape tile (0 otherwise). Tiles: with esc_idx[tile] = the tile's escape entry or -1, writes the planes, the rest of the
+// header and the escape tiles' exponent planes into esc.
+cudaError_t launch_pack_scan(const bf16* src, int N, int K, int mode, int hd, uint8_t* dst, uint8_t* escape, cudaStream_t s);
+cudaError_t launch_pack_tiles(const bf16* src, int N, int K, int mode, int hd, const int* esc_idx, uint8_t* dst, uint8_t* esc,
+                              cudaStream_t s);
 
 // device image preprocessing (Pillow-exact 8-bit bicubic resize + rescale + normalise): rgb uint8 [h, w, 3] -> fp32 [3, S, S]
 cudaError_t launch_image_preprocess(const uint8_t* rgb, int h, int w, int S, const int* bounds_h, const int* coef_h, int ksize_h,

@@ -240,7 +240,8 @@ class Engine:
 
     def decode_bytes(self, context_len: int) -> int:
         """HBM bytes of one batch-1 decode step at ``context_len``: the weight bytes the persistent kernel streams in the
-        current mode (option ``decode_weight_bytes``: e4m3 layer matrices with ``decode_fp8``) plus the cached keys/values."""
+        current mode (option ``decode_weight_bytes``: e4m3 layer matrices with ``decode_fp8``, 13-bit packed tiles with
+        ``decode_pack``) plus the cached keys/values."""
         kv = self.lib.dtk_decode_bytes(C.byref(self.ccfg), context_len) - self.lib.dtk_decode_bytes(C.byref(self.ccfg), 0)
         return self.get_option("decode_weight_bytes") + int(kv)
 

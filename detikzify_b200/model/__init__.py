@@ -116,7 +116,8 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
     computes the same quantized model, and batch-1 decode and batched decode steps of 4 <= B < 64 rows (rollouts,
     ``generate_batch``) stream the layer matrices as e4m3 (about half the bytes) with bit-identical logits.
     Embeddings, norms, lm_head, projector, vision tower and KV cache stay bf16. ``None`` (default) keeps the weights as
-    they are.
+    they are, and batch-1 decode streams them as lossless 13-bit packed tiles (engine option ``decode_pack``: the same
+    logits as bf16 tiles, about 17 % fewer bytes per token).
     """
     from ..engine import pack_arena, to_c_config, weight_table
     from ..quant import quantize_arena_fp8
@@ -178,7 +179,7 @@ def load(model_name_or_path, modality_projector: Optional[str] = None, is_v1: bo
         dist.broadcast(arena, src=0)  # the single collective of the whole path
 
     model = DetikzifyForCausalLM(cfg, arena, device=device, dtype=dtype, max_seqs=max_seqs, max_batch=max_batch,
-                                 prefix_slots=prefix_slots)
+                                 prefix_slots=prefix_slots, decode_pack=quantize != "fp8")
     if quantize == "fp8":
         model.engine.set_option("decode_fp8", 1)
     tokenizer = _load_tokenizer(model_name_or_path, cfg) if is_dir else None

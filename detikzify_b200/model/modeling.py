@@ -118,7 +118,7 @@ class _KVSlot:
 class DetikzifyForCausalLM:
     def __init__(self, config: DetikzifyConfig, arena: Optional[torch.Tensor] = None, device=0, dtype=torch.bfloat16,
                  max_seqs: int = 2, max_batch: int = 1, max_len: Optional[int] = None, engine=None,
-                 prefix_slots: Optional[int] = None):
+                 prefix_slots: Optional[int] = None, decode_pack: bool = False):
         self.config = config
         self.dtype = dtype
         self.name_or_path = config.name_or_path
@@ -127,6 +127,9 @@ class DetikzifyForCausalLM:
         self.engine = engine if engine is not None else Engine(config, arena, device=device, max_seqs=max_seqs,
                                                                 max_batch=max_batch, max_len=max_len)
         self.device = self.engine.device
+        # decode_pack: batch-1 decode streams the weights as lossless 13-bit packed tiles (same logits, fewer bytes per token)
+        if decode_pack and engine is None and self.engine.get_option("decode_persistent"):
+            self.engine.set_option("decode_pack", 1)
         self.generation_config = GenerationConfig(
             max_length=config.model_max_length, do_sample=False, temperature=1.0, top_p=1.0, top_k=0,
             bos_token_id=config.bos_token_id, eos_token_id=config.eos_token_id, pad_token_id=config.pad_token_id)

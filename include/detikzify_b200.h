@@ -230,11 +230,15 @@ DTK_API int dtk_gen_end(dtk_engine* eng);
  *      4 <= B < 64 stream the four decoder-layer matrices as e4m3 codes plus one power-of-two exponent per row
  *      (rebuilt from the arena, whose every row must be e4m3 x 2^k; otherwise DTK_ERR_INVALID names the layer
  *      and matrix and nothing changes), 0 (default) = bf16. The logits equal the bf16 kernels' on the same
- *      arena; B = 2, 3, B >= 64 and the lm_head always run bf16. --------------------------------------- */
+ *      arena; B = 2, 3, B >= 64 and the lm_head always run bf16.
+ *      "decode_pack": 1 = the persistent kernel (B = 1) streams every matrix, lm_head included, as lossless 13-bit
+ *      packed tiles (any bf16 weights; the logits equal the bf16 tiles'), 0 (default of dtk_create) = bf16 tiles.
+ *      bf16, e4m3 and packed tiles are exclusive: setting one of decode_fp8 / decode_pack to 1 clears the other. */
 DTK_API int dtk_set_option(dtk_engine* eng, const char* key, int64_t value);
 /*      Read back an option; the extra key "decode_persistent" reports whether B = 1 decode steps
  *      actually run on the persistent kernel (option set AND the device can co-schedule its grid), and
- *      "decode_weight_bytes" the weight bytes one such step streams in the current mode (lm_head in bf16). */
+ *      "decode_weight_bytes" the weight bytes one such step streams in the current mode (packed: tiles and escape
+ *      planes; otherwise the lm_head in bf16), "decode_pack_escapes" the packed weights' escape tiles. */
 DTK_API int dtk_get_option(dtk_engine* eng, const char* key, int64_t* value);
 
 /* ---- introspection for benches: algorithmic HBM bytes of one decode step at context T ----- */
@@ -251,6 +255,9 @@ DTK_API int dtk_dbg_mega_times(dtk_engine* eng, long long* out_host, int max_val
  * rows 0..159 = the CTA's local tiles of that layer {producer issue, bytes landed, tile done, consumer asked},
  * rows 160..164 = the layer's five phases {start, staged, items done, barrier done}; returns the value count */
 DTK_API int dtk_dbg_mega_trace(dtk_engine* eng, long long* out_host, int max_values);
+/* bytes [offset, offset + nbytes) of the packed decode tiles (option "decode_pack" = 1): [layer][wqkv | wo | wgu | wd tiles],
+ * then the lm_head tiles, 6688 bytes per tile (launch.h, MegaPack) */
+DTK_API int dtk_dbg_pack_bytes(dtk_engine* eng, int64_t offset, int64_t nbytes, void* out_host);
 /* select the dense GEMM implementation used by dtk_dbg_gemm and the engines of this process:
  * 0 = mma.sync, 1 = wgmma one 128 x 128 tile per CTA, 2 (default) = persistent 128 x 256 wgmma kernel,
  * -1 = query only; returns the current setting. Bits 8..11 of a

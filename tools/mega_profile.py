@@ -1,16 +1,20 @@
 """Phase-level timeline of the persistent decode kernel across all CTAs (dev tool).
-Usage: python tools/mega_profile.py [--fp8] [model] [ctx] [trace.pt]  (the trace goes to the temporary directory by default;
---fp8: weights quantized as load(..., quantize="fp8") does, decode on the FP8 layer tiles)."""
+Usage: python tools/mega_profile.py [--fp8 | --bf16] [model] [ctx] [trace.pt]  (the trace goes to the temporary directory by
+default; the decode streams packed tiles as load() sets them up; --fp8: weights quantized as load(..., quantize="fp8") does,
+decode on the FP8 layer tiles; --bf16: decode on bf16 tiles)."""
 import ctypes as C, os, sys, tempfile
 import torch
 sys.path.insert(0, ".")
 from detikzify_b200.model import load
-fp8 = "--fp8" in sys.argv
-sys.argv = [a for a in sys.argv if a != "--fp8"]
+fp8, bf16 = "--fp8" in sys.argv, "--bf16" in sys.argv
+sys.argv = [a for a in sys.argv if a not in ("--fp8", "--bf16")]
 name = sys.argv[1] if len(sys.argv) > 1 else "nllg/detikzify-ds-1.3b"
 ctx = int(sys.argv[2]) if len(sys.argv) > 2 else 1000
 model, _ = load(name, device_map=0, quantize="fp8" if fp8 else None)
 eng, cfg = model.engine, model.config
+if bf16:
+    eng.set_option("decode_pack", 0)
+print(f"tile format: {'fp8' if eng.get_option('decode_fp8') else 'packed' if eng.get_option('decode_pack') else 'bf16'}")
 slot = eng.seq_alloc()
 g = torch.Generator().manual_seed(1)
 ids = torch.randint(0, 30000, (ctx,), generator=g).cuda()
