@@ -910,13 +910,18 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
   return DTK_OK;
 }
 
-void fill_sample_args(dtk_engine* eng, SampleArgs& a, const float* logits, int B, const dtk_sampling& p) {
+// the sampling rules of dtk_sampling, shared by the engine's sampler and the engine-free test hook dtk_dbg_sample
+void fill_sample_params(SampleArgs& a, const float* logits, int B, int V, const dtk_sampling& p) {
   std::memset(&a, 0, sizeof(a));
-  a.logits = logits; a.B = B; a.V = eng->cfg.vocab;
+  a.logits = logits; a.B = B; a.V = V;
   a.temperature = (float)p.temperature; a.top_p = (float)p.top_p; a.top_p_limit = (float)(1.0 - p.top_p); a.top_k = p.top_k;
-  a.max_pos = eng->cfg.max_len - 1;
   a.do_sample = (p.do_sample && p.temperature >= 1e-5) ? 1 : 0;
   a.bad_token = p.bad_token; a.bs_token = p.begin_suppress_token; a.seed = p.seed;
+}
+
+void fill_sample_args(dtk_engine* eng, SampleArgs& a, const float* logits, int B, const dtk_sampling& p) {
+  fill_sample_params(a, logits, B, eng->cfg.vocab, p);
+  a.max_pos = eng->cfg.max_len - 1;
   a.scratch = eng->d_scratch;
 }
 
@@ -1885,6 +1890,25 @@ int dtk_dbg_gemm_impl(int impl) {
     set_gemm_swap_split((impl >> 8) & 0xf);   // forced split-K factor of the batched-decode tile (0 = heuristic)
   }
   return get_gemm_impl();
+}
+
+int dtk_dbg_sample(const float* logits, int B, int V, const dtk_sampling* params, const int* suppress, const uint32_t* steps,
+                   const uint32_t* seq_ids, int impl, int64_t* out_ids, float* probs, void* stream) {
+  if (!logits || !params || !out_ids || !probs || B < 1 || B > 64 || V < 1 || (impl != 0 && impl != 1)) return DTK_ERR_INVALID;
+  SampleArgs a;
+  fill_sample_params(a, logits, B, V, *params);
+  a.scratch = probs; a.want_probs = 1;
+  a.out_ids = out_ids;
+  for (int i = 0; i < B; ++i) {
+    a.seq[i].suppress = suppress ? suppress[i] : 0;
+    a.seq[i].step = steps ? steps[i] : 0;
+    a.seq[i].seq_id = seq_ids ? seq_ids[i] : (uint32_t)i;
+  }
+  const int prev = get_sample_impl();
+  set_sample_impl(impl);
+  const cudaError_t e = launch_sample(a, (cudaStream_t)stream, nullptr);
+  set_sample_impl(prev);
+  return e == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
 }
 
 int dtk_dbg_gemm(const void* A, const void* Wm, const void* bias, const float* resid, int M, int N, int K, int act,

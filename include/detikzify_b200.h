@@ -272,6 +272,14 @@ DTK_API int dtk_dbg_gemm(const void* A_bf16, const void* W_bf16, const void* bia
  * calls must not overlap. */
 DTK_API int dtk_dbg_lm_logprob(const void* A_bf16, const void* W_bf16, int M, int N, int K, const int64_t* targets,
                                float* logprob, float* lse, void* stream);
+/* the sampler of dtk_sample without an engine, at any vocabulary size: logits fp32 [B,V], 1 <= B <= 64, V >= 1; suppress,
+ * steps, seq_ids host arrays [B] as in dtk_sample (NULL = 0, 0, b); impl 0 = dtk_sample's dispatch (register-resident kernel
+ * while V <= 32768), 1 = the generic kernel (the process-wide "sample_impl" setting is restored afterwards); out_ids int64 [B];
+ * probs fp32 [B,V] (required) receives the probability vector the token was drawn from (softmax of the masked logits when
+ * greedy) */
+DTK_API int dtk_dbg_sample(const float* logits, int B, int V, const dtk_sampling* params, const int* suppress,
+                           const uint32_t* steps, const uint32_t* seq_ids, int impl, int64_t* out_ids, float* probs,
+                           void* stream);
 /* q,k,v,o bf16 [B, T, heads, head_dim]; head_dim in {72,128} */
 DTK_API int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void* o, int B,
                                int heads, int Tq, int Tk, int head_dim, int causal, int q_pos0,
