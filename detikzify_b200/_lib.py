@@ -46,6 +46,13 @@ class DtkSampling(C.Structure):
                 ("seed", C.c_uint64)]
 
 
+class DtkProcessors(C.Structure):
+    _fields_ = [("repetition_penalty", C.c_double), ("min_p", C.c_double), ("no_repeat_ngram_size", C.c_int32),
+                ("eos_token_id", C.c_int32), ("ban_ids", C.POINTER(C.c_int32)), ("n_ban", C.c_int32),
+                ("begin_ids", C.POINTER(C.c_int32)), ("n_begin", C.c_int32), ("word_ids", C.POINTER(C.c_int32)),
+                ("word_lens", C.POINTER(C.c_int32)), ("n_words", C.c_int32)]
+
+
 # every symbol include/detikzify_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -76,6 +83,8 @@ SYMBOLS = {
     "dtk_decode": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, C.c_int, _P, _P]),
     "dtk_sample": (C.c_int, [_P, _P, C.c_int, C.POINTER(DtkSampling), C.POINTER(C.c_int),
                              C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), _P, _P, _P]),
+    "dtk_set_processors": (C.c_int, [_P, C.POINTER(DtkProcessors), C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                     C.POINTER(C.c_int32), _P]),
     "dtk_gen_begin": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64), C.c_int,
                                 C.POINTER(DtkSampling), C.POINTER(C.c_uint32), _P]),
     "dtk_gen_step": (C.c_int, [_P, _P]),
@@ -92,6 +101,9 @@ SYMBOLS = {
     "dtk_dbg_gemm": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "dtk_dbg_sample": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(DtkSampling), C.POINTER(C.c_int), C.POINTER(C.c_uint32),
                                  C.POINTER(C.c_uint32), C.c_int, _P, _P, _P]),
+    "dtk_dbg_sample_proc": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(DtkSampling), C.POINTER(C.c_int),
+                                      C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_int, C.POINTER(DtkProcessors),
+                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, _P, _P, _P]),
     "dtk_dbg_lm_logprob": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
     "dtk_dbg_flash_attn": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_float, _P]),

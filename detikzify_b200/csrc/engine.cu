@@ -246,6 +246,12 @@ struct dtk_engine {
   bool gen_fused = false;    // greedy generation on the persistent kernel: argmax + token publication in the kernel tail
   unsigned long long* d_amax = nullptr;
   SampleArgs gen_sample{};
+  // HF logits processors (dtk_set_processors): tables and per-row token histories in engine-owned device buffers
+  SampleProcTable* d_proc_tab = nullptr;
+  int* d_hist = nullptr;                // [max_batch][max_len]
+  int* d_hist_len = nullptr;            // [max_batch]
+  int proc_B = 0;                       // rows set by the last dtk_set_processors; 0 = processors off
+  bool gen_proc = false;                // the generation loop runs the processor instantiation of the sampler
   unsigned long long* d_bar = nullptr;  // [0] counter, [1] epoch base
   unsigned int* d_head_cnt = nullptr;
   bf16* d_tiled = nullptr;             // decode-side re-tiled copy of the four layer matrices (bf16 mode)
@@ -925,6 +931,61 @@ void fill_sample_args(dtk_engine* eng, SampleArgs& a, const float* logits, int B
   a.scratch = eng->d_scratch;
 }
 
+// host image of the processor table for B rows: validates dtk_processors (HF's argument checks) and the histories
+bool fill_proc_table(const dtk_processors& p, int B, int V, int max_len, const int32_t* hist_ids, const int32_t* hist_len,
+                     const int32_t* eos_min_len, SampleProcTable& t, std::vector<int>& hist, std::string& why) {
+  std::memset(&t, 0, sizeof(t));
+  if (!(p.repetition_penalty > 0.0) || !std::isfinite(p.repetition_penalty)) { why = "repetition_penalty must be a positive float"; return false; }
+  if (p.no_repeat_ngram_size < 0) { why = "no_repeat_ngram_size must be >= 0"; return false; }
+  if (!(p.min_p >= 0.0 && p.min_p <= 1.0)) { why = "min_p must lie in [0, 1]"; return false; }
+  if (p.n_ban < 0 || p.n_begin < 0 || p.n_words < 0) { why = "negative table size"; return false; }
+  if ((p.n_ban && !p.ban_ids) || (p.n_begin && !p.begin_ids) || (p.n_words && (!p.word_ids || !p.word_lens))) { why = "null table"; return false; }
+  if (V > kProcMaxVocab) { why = "logits processors need vocab <= " + std::to_string(kProcMaxVocab); return false; }
+  auto id_ok = [&](int id) { return id >= 0 && id < V; };
+  if (p.eos_token_id != -1 && !id_ok(p.eos_token_id)) { why = "eos_token_id outside [0, vocab)"; return false; }
+  int64_t nword_ids = 0;
+  for (int e = 0; e < p.n_words; ++e) {
+    if (p.word_lens[e] < 2) { why = "bad-word sequences in word_ids must hold >= 2 ids (single ids go to ban_ids)"; return false; }
+    nword_ids += p.word_lens[e];
+  }
+  const int64_t total = (int64_t)p.n_ban + p.n_begin + p.n_words + 1 + nword_ids;
+  if (total > kProcMaxIds) { why = "processor tables exceed " + std::to_string(kProcMaxIds) + " ids (ban + begin + bad-word ids + bad-word count + 1)"; return false; }
+  t.penalty = (float)p.repetition_penalty; t.min_p = (float)p.min_p; t.ngram = p.no_repeat_ngram_size; t.eos = p.eos_token_id;
+  t.n_ban = p.n_ban; t.n_begin = p.n_begin; t.n_words = p.n_words;
+  int k = 0;
+  for (int i = 0; i < p.n_ban; ++i) { if (!id_ok(p.ban_ids[i])) { why = "ban id outside [0, vocab)"; return false; } t.ids[k++] = p.ban_ids[i]; }
+  for (int i = 0; i < p.n_begin; ++i) { if (!id_ok(p.begin_ids[i])) { why = "begin-suppress id outside [0, vocab)"; return false; } t.ids[k++] = p.begin_ids[i]; }
+  int o = 0;
+  for (int e = 0; e <= p.n_words; ++e) { t.ids[k++] = o; if (e < p.n_words) o += p.word_lens[e]; }
+  for (int i = 0; i < nword_ids; ++i) { if (!id_ok(p.word_ids[i])) { why = "bad-word id outside [0, vocab)"; return false; } t.ids[k++] = p.word_ids[i]; }
+  hist.assign((size_t)B * max_len, 0);
+  int64_t at = 0;
+  for (int b = 0; b < B; ++b) {
+    const int L = hist_len ? hist_len[b] : 0;
+    if (L < 0 || L > max_len) { why = "history length outside [0, max_len]"; return false; }
+    for (int i = 0; i < L; ++i) {
+      const int id = hist_ids[at + i];
+      if (!id_ok(id)) { why = "history id outside [0, vocab)"; return false; }
+      hist[(size_t)b * max_len + i] = id;
+    }
+    at += L;
+    t.eos_until[b] = eos_min_len ? eos_min_len[b] : 0;
+  }
+  return true;
+}
+
+SampleProc proc_args(dtk_engine* eng) {
+  SampleProc q{};
+  q.tab = eng->d_proc_tab; q.hist = eng->d_hist; q.hist_len = eng->d_hist_len; q.hist_stride = eng->cfg.max_len;
+  return q;
+}
+
+// the generation loop's sampler launch: the processor instantiation while processors are set at dtk_gen_begin
+cudaError_t launch_gen_sample(dtk_engine* eng, cudaStream_t s) {
+  return eng->gen_proc ? launch_sample_proc(eng->gen_sample, proc_args(eng), s, &eng->launches)
+                       : launch_sample(eng->gen_sample, s, &eng->launches);
+}
+
 }  // namespace
 
 // ================================================================== C ABI
@@ -1101,7 +1162,8 @@ int dtk_destroy(dtk_engine* eng) {
   void* ptrs[] = {eng->v_pix_in, eng->v_tok_out, eng->v_pool_out, eng->v_vt, eng->kv, eng->rope_cs, eng->p_x, eng->p_qkv, eng->p_xn, eng->p_q, eng->p_att, eng->p_h, eng->d_x, eng->d_q,
                   eng->d_att, eng->d_h, eng->d_logits, eng->d_scratch, eng->d_part_o, eng->d_part_ml, eng->d_counters,
                   eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tiled_lm, eng->d_tiled8, eng->d_tiledpk, eng->d_pk_esc, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
-                  eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt};
+                  eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt, eng->d_proc_tab, eng->d_hist,
+                  eng->d_hist_len};
   for (void* p : ptrs) if (p) cudaFree(p);
   dtk_adapter_detach(eng);
   if (eng->cap_stream) cudaStreamDestroy(eng->cap_stream);
@@ -1601,7 +1663,47 @@ int dtk_sample(dtk_engine* eng, const float* logits, int B, const dtk_sampling* 
     a.seq[i].step = steps ? steps[i] : 0;
     a.seq[i].seq_id = seq_ids ? seq_ids[i] : (uint32_t)i;
   }
-  DTK_CK(launch_sample(a, (cudaStream_t)stream, &eng->launches));
+  if (eng->proc_B > 0) {
+    DTK_REQUIRE(B <= eng->proc_B, "B exceeds the rows given to dtk_set_processors");
+    DTK_CK(launch_sample_proc(a, proc_args(eng), (cudaStream_t)stream, &eng->launches));
+  } else {
+    DTK_CK(launch_sample(a, (cudaStream_t)stream, &eng->launches));
+  }
+  return DTK_OK;
+}
+
+int dtk_set_processors(dtk_engine* eng, const dtk_processors* proc, int B, const int32_t* hist_ids, const int32_t* hist_len,
+                       const int32_t* eos_min_len, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->gen_B == 0, "processors cannot change inside a generation loop");
+  if (!proc) { eng->proc_B = 0; return DTK_OK; }
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(B > 0 && B <= c.max_batch && B <= 64, "B outside [1, max_batch]");
+  DTK_REQUIRE(hist_len, "null history lengths");
+  int64_t n = 0;
+  for (int b = 0; b < B; ++b) n += hist_len[b] > 0 ? hist_len[b] : 0;
+  DTK_REQUIRE(n == 0 || hist_ids, "null history ids");
+  SampleProcTable t;
+  std::vector<int> hist;
+  std::string why;
+  if (!fill_proc_table(*proc, B, c.vocab, c.max_len, hist_ids, hist_len, eos_min_len, t, hist, why)) {
+    eng->err = "invalid argument: " + why;
+    return DTK_ERR_INVALID;
+  }
+  DTK_CK(cudaSetDevice(eng->device));
+  if (!eng->d_proc_tab) {
+    DTK_ALLOC(eng->d_proc_tab, 1);
+    DTK_ALLOC(eng->d_hist, (int64_t)c.max_batch * c.max_len);
+    DTK_ALLOC(eng->d_hist_len, c.max_batch);
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<int> lens(hist_len, hist_len + B);
+  // pageable sources: the copies are staged before the calls return, so the host vectors may go out of scope
+  DTK_CK(cudaMemcpyAsync(eng->d_proc_tab, &t, sizeof(t), cudaMemcpyHostToDevice, s));
+  DTK_CK(cudaMemcpyAsync(eng->d_hist, hist.data(), hist.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  DTK_CK(cudaMemcpyAsync(eng->d_hist_len, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  DTK_CK(cudaStreamSynchronize(s));
+  eng->proc_B = B;
   return DTK_OK;
 }
 
@@ -1642,8 +1744,11 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
     a.host_ring = eng->dev_ring; a.ring = eng->ring;
     a.done_counter = eng->d_counters + (int64_t)c.max_batch * c.heads;
   }
+  DTK_REQUIRE(eng->proc_B == 0 || B <= eng->proc_B, "B exceeds the rows given to dtk_set_processors");
+  eng->gen_proc = eng->proc_B > 0;
   eng->gen_mega = (B == 1 && eng->decode_impl == 1 && eng->mega_ok);
-  eng->gen_fused = eng->gen_mega && eng->fuse_greedy && !eng->gen_sample.do_sample;
+  // the fused argmax of the persistent kernel knows only the bad token: processors take the token from the sampler
+  eng->gen_fused = eng->gen_mega && eng->fuse_greedy && !eng->gen_sample.do_sample && !eng->gen_proc;
   if (eng->gen_mega) {  // one cooperative launch (+ sampler when sampling) per token: no graph needed
     eng->gen_graph = nullptr;
     return DTK_OK;
@@ -1655,6 +1760,7 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
   std::string skey(key);
   skey += "|g" + std::to_string(eng->decode_gemm_min_batch) + "|i" + std::to_string(get_gemm_impl());
   skey += "|c" + std::to_string(eng->cas_slot) + ":" + std::to_string(eng->cas_len);   // shared-prefix attention bakes slot and length in
+  if (eng->gen_proc) skey += "|P";   // processor tables and histories are read from engine buffers at replay
   if (seq_ids) for (int i = 0; i < B; ++i) skey += "," + std::to_string(seq_ids[i]);
   auto it = eng->graphs.find(skey);
   if (it == eng->graphs.end()) {
@@ -1665,7 +1771,7 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
     DTK_CK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
     int r = decode_launches(eng, B, nullptr, eng->d_logits, cs);
     if (r == DTK_OK) {
-      cudaError_t e = launch_sample(eng->gen_sample, cs, &eng->launches);
+      cudaError_t e = launch_gen_sample(eng, cs);
       if (e != cudaSuccess) { eng->err = std::string("launch_sample: ") + cudaGetErrorString(e); r = DTK_ERR_CUDA; }
     }
     cudaError_t ce = cudaStreamEndCapture(cs, &graph);
@@ -1691,7 +1797,7 @@ int dtk_gen_step(dtk_engine* eng, void* stream) {
   if (eng->gen_mega) {
     int r = decode_launches(eng, 1, nullptr, eng->d_logits, (cudaStream_t)stream);
     if (r != DTK_OK) return r;
-    if (!eng->gen_fused) DTK_CK(launch_sample(eng->gen_sample, (cudaStream_t)stream, &eng->launches));
+    if (!eng->gen_fused) DTK_CK(launch_gen_sample(eng, (cudaStream_t)stream));
     return DTK_OK;
   }
   DTK_REQUIRE(eng->gen_graph != nullptr, "dtk_gen_begin not called");
@@ -1746,6 +1852,7 @@ int dtk_gen_end(dtk_engine* eng) {
   eng->gen_graph = nullptr;
   eng->gen_mega = false;
   eng->gen_fused = false;
+  eng->gen_proc = false;
   eng->gen_B = 0;
   return DTK_OK;
 }
@@ -1908,6 +2015,46 @@ int dtk_dbg_sample(const float* logits, int B, int V, const dtk_sampling* params
   set_sample_impl(impl);
   const cudaError_t e = launch_sample(a, (cudaStream_t)stream, nullptr);
   set_sample_impl(prev);
+  return e == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
+}
+
+int dtk_dbg_sample_proc(const float* logits, int B, int V, const dtk_sampling* params, const int* suppress, const uint32_t* steps,
+                        const uint32_t* seq_ids, int impl, const dtk_processors* proc, const int32_t* hist_ids,
+                        const int32_t* hist_len, const int32_t* eos_min_len, int max_len, int64_t* out_ids, float* probs,
+                        void* stream) {
+  if (!logits || !params || !proc || !hist_len || !out_ids || !probs || B < 1 || B > 64 || V < 1 || max_len < 1 ||
+      (impl != 0 && impl != 1))
+    return DTK_ERR_INVALID;
+  SampleProcTable t;
+  std::vector<int> hist;
+  std::string why;
+  if (!fill_proc_table(*proc, B, V, max_len, hist_ids, hist_len, eos_min_len, t, hist, why)) return DTK_ERR_INVALID;
+  SampleArgs a;
+  fill_sample_params(a, logits, B, V, *params);
+  a.scratch = probs; a.want_probs = 1;
+  a.out_ids = out_ids;
+  for (int i = 0; i < B; ++i) {
+    a.seq[i].suppress = suppress ? suppress[i] : 0;
+    a.seq[i].step = steps ? steps[i] : 0;
+    a.seq[i].seq_id = seq_ids ? seq_ids[i] : (uint32_t)i;
+  }
+  SampleProc q{};
+  q.hist_stride = max_len;
+  cudaError_t e = cudaMalloc((void**)&q.tab, sizeof(SampleProcTable));
+  if (e == cudaSuccess) e = cudaMalloc((void**)&q.hist, hist.size() * sizeof(int));
+  if (e == cudaSuccess) e = cudaMalloc((void**)&q.hist_len, B * sizeof(int));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (e == cudaSuccess) e = cudaMemcpyAsync((void*)q.tab, &t, sizeof(t), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(q.hist, hist.data(), hist.size() * sizeof(int), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(q.hist_len, hist_len, B * sizeof(int), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) {
+    const int prev = get_sample_impl();
+    set_sample_impl(impl);
+    e = launch_sample_proc(a, q, s, nullptr);
+    set_sample_impl(prev);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);   // the temporary tables are freed below
+  cudaFree((void*)q.tab); cudaFree(q.hist); cudaFree(q.hist_len);
   return e == cudaSuccess ? DTK_OK : DTK_ERR_CUDA;
 }
 

@@ -221,6 +221,28 @@ struct SampleArgs {
   SampleSeq seq[64];
 };
 cudaError_t launch_sample(const SampleArgs& a, cudaStream_t s, uint64_t* counter);
+// HF logits processors beyond one bad token and one begin-suppress token (dtk_processors): the tables live in device
+// memory, so a captured graph bakes only the pointers. Every CTA builds a ban bitmask and a repetition-penalty bitmask of
+// its row in shared memory (2 x 16 KB, so V <= kProcMaxVocab) from the row's token history and the tables.
+constexpr int kProcMaxIds = 4096;
+constexpr int kProcMaxVocab = 131072;
+struct SampleProcTable {
+  float penalty;       // repetition penalty (1 = off)
+  float min_p;         // 0 = off; applied only when sampling
+  int ngram;           // no_repeat_ngram_size (0 = off)
+  int eos;             // id banned while a row's history is shorter than eos_until[row] (-1 = none)
+  int n_ban, n_begin, n_words, pad;
+  int eos_until[64];
+  // ban ids [n_ban] | begin-suppress ids [n_begin] | bad-word offsets [n_words + 1] (relative to the word ids) | word ids
+  int ids[kProcMaxIds];
+};
+struct SampleProc {
+  const SampleProcTable* tab;   // device
+  int* hist;                    // device int32 [B][hist_stride]: each row's prompt + tokens so far
+  int* hist_len;                // device int32 [B]; the generation loop appends the drawn token (clamped at hist_stride)
+  int hist_stride;
+};
+cudaError_t launch_sample_proc(const SampleArgs& a, const SampleProc& q, cudaStream_t s, uint64_t* counter);
 void set_sample_impl(int impl);   // 0 = register-resident kernel when V <= 32768 (default), 1 = generic kernel
 int get_sample_impl();
 

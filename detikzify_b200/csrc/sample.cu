@@ -8,6 +8,10 @@
 // The full-vocabulary sort of HF's TopP warper is replaced by a bit-wise threshold search on the
 // float pattern of the probabilities (31 block reductions): tokens with ascending-cumulative mass
 // <= 1 - top_p are removed, exactly HF's rule (ties are kept or dropped together).
+// The PROC instantiations (dtk_processors) add HF's other processors in HF's order:
+//   repetition penalty -> no-repeat n-gram -> bad words -> min length / min new tokens -> suppress tokens ->
+//   begin-suppress tokens -> /T -> top-k -> softmax -> top-p -> min-p -> renormalise -> draw;
+// the instantiations without them compile to the same code as before.
 #include "common.cuh"
 #include "launch.h"
 
@@ -99,7 +103,66 @@ DTK_DEV float philox_uniform(uint64_t seed, uint32_t c0, uint32_t c1) {
   return (float)(x0 >> 8) * (1.0f / 16777216.0f);
 }
 
-__global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) {
+// ---- HF logits processors (sampler instantiations with PROC = true only): the ban and repetition-penalty bitmasks of row
+// b, built from its token history h[0, L) and the call's tables in shared memory (2 x 4096 words, so V <= 131072).
+// HF generation/logits_process.py: RepetitionPenalty (every distinct id of input_ids), NoRepeatNGram
+// (_calc_banned_ngram_tokens), NoBadWords (SequenceBias with -inf: length-1 entries always, a longer entry when the history
+// ends with its prefix, skipped when longer than the history), MinLength / MinNewTokensLength (EOS), SuppressTokens,
+// SuppressTokensAtBegin (first new token: the suppress flag).
+DTK_DEV void set_bit(uint32_t* m, int id, int V) {
+  if ((unsigned)id < (unsigned)V) atomicOr(m + (id >> 5), 1u << (id & 31));
+}
+DTK_DEV bool get_bit(const uint32_t* m, int id) { return (m[id >> 5] >> (id & 31)) & 1u; }
+
+DTK_DEV void build_proc_masks(const SampleProc& q, int b, int suppress, int V, uint32_t* ban, uint32_t* pen) {
+  const int tid = threadIdx.x, nw = (V + 31) >> 5;
+  for (int i = tid; i < nw; i += ST) { ban[i] = 0u; pen[i] = 0u; }
+  __syncthreads();
+  const SampleProcTable& t = *q.tab;
+  const int L = q.hist_len[b];
+  const int* h = q.hist + (int64_t)b * q.hist_stride;
+  if (t.penalty != 1.f)
+    for (int i = tid; i < L; i += ST) set_bit(pen, h[i], V);
+  for (int i = tid; i < t.n_ban; i += ST) set_bit(ban, t.ids[i], V);
+  if (suppress)
+    for (int i = tid; i < t.n_begin; i += ST) set_bit(ban, t.ids[t.n_ban + i], V);
+  if (tid == 0 && L < t.eos_until[b]) set_bit(ban, t.eos, V);
+  const int n = t.ngram;
+  if (n > 0 && L + 1 >= n) {   // every n-gram h[j, j + n) whose first n - 1 ids equal the last n - 1 ids bans h[j + n - 1]
+    const int* tail = h + (L - n + 1);
+    for (int j = tid; j <= L - n; j += ST) {
+      bool eq = true;
+      for (int k = 0; k < n - 1 && eq; ++k) eq = h[j + k] == tail[k];
+      if (eq) set_bit(ban, h[j + n - 1], V);
+    }
+  }
+  const int* off = t.ids + t.n_ban + t.n_begin;
+  const int* wid = off + t.n_words + 1;
+  for (int e = tid; e < t.n_words; e += ST) {
+    const int o0 = off[e], len = off[e + 1] - o0;
+    if (len > L) continue;
+    bool eq = true;
+    for (int k = 0; k < len - 1 && eq; ++k) eq = h[L - len + 1 + k] == wid[o0 + k];
+    if (eq) set_bit(ban, wid[o0 + len - 1], V);
+  }
+  __syncthreads();
+}
+
+// repetition penalty in fp32 on the raw logit, then the bans (before the division by T)
+DTK_DEV float apply_proc(float x, int i, float penalty, const uint32_t* ban, const uint32_t* pen) {
+  if (get_bit(pen, i)) x = x < 0.f ? __fmul_rn(x, penalty) : __fdiv_rn(x, penalty);
+  return get_bit(ban, i) ? -INFINITY : x;
+}
+
+// the generation loop appends the drawn token to the row's history, clamped at the row's end as gen_pos is at max_pos
+DTK_DEV void append_hist(const SampleProc& q, int b, int token) {
+  const int L = q.hist_len[b];
+  if (L < q.hist_stride) q.hist[(int64_t)b * q.hist_stride + L] = token;
+  q.hist_len[b] = min(L + 1, q.hist_stride);
+}
+
+template <bool PROC>
+DTK_DEV void sample_generic_body(const SampleArgs p, const SampleProc q) {
   __shared__ RedScratch red;
   __shared__ float sm_scan[32];
   __shared__ int sm_choice;
@@ -110,12 +173,23 @@ __global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) 
   const bool sampling = p.do_sample && p.temperature > 0.f;
   const float T = sampling ? p.temperature : 1.f;
   unsigned long long gstep = p.gen_step ? *p.gen_step : 0ull;
+  uint32_t *ban = nullptr, *pen = nullptr;
+  float penalty = 1.f, min_p = 0.f;
+  if constexpr (PROC) {
+    __shared__ uint32_t proc_masks[2 * (kProcMaxVocab / 32)];
+    ban = proc_masks;
+    pen = proc_masks + ((V + 31) >> 5);
+    build_proc_masks(q, b, sq.suppress, V, ban, pen);
+    penalty = q.tab->penalty;
+    min_p = q.tab->min_p;
+  }
 
   // 1. masks + temperature, running (max, argmax)
   float mx = -INFINITY;
   int amx = 0x7fffffff;
   for (int i = tid; i < V; i += ST) {
     float v = lg[i];
+    if constexpr (PROC) v = apply_proc(v, i, penalty, ban, pen);
     if (i == p.bad_token || (sq.suppress && i == p.bs_token)) v = -INFINITY;
     v = v / T;
     w[i] = v;
@@ -170,12 +244,21 @@ __global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) 
       const float pmax = invz;  // exp(0) / z
       if (theta >= pmax) theta = nextafterf(pmax, 0.f);  // min_tokens_to_keep = 1
     }
-    // 5. renormalise over the nucleus
+    // 5. renormalise over the nucleus (min-p: also drop p < min_p * p_max; p_max = invz is always kept)
     float z2 = 0.f;
-    for (int i = tid; i < V; i += ST) {
-      float pv = w[i];
-      if (pv <= theta) { pv = 0.f; w[i] = 0.f; }
-      z2 += pv;
+    if constexpr (PROC) {
+      const float mthr = min_p * invz;
+      for (int i = tid; i < V; i += ST) {
+        float pv = w[i];
+        if (pv <= theta || pv < mthr) { pv = 0.f; w[i] = 0.f; }
+        z2 += pv;
+      }
+    } else {
+      for (int i = tid; i < V; i += ST) {
+        float pv = w[i];
+        if (pv <= theta) { pv = 0.f; w[i] = 0.f; }
+        z2 += pv;
+      }
     }
     z2 = block_sum(z2, red);
     const float invz2 = 1.f / z2;
@@ -242,6 +325,7 @@ __global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) 
     if (p.gen_tok) {
       p.gen_tok[b] = token;
       p.gen_pos[b] = min(p.gen_pos[b] + 1, p.max_pos);
+      if constexpr (PROC) append_hist(q, b, token);
       // ONE 8-byte store to the mapped pinned ring carries the token and its step stamp, so no ordering between two
       // host-visible stores (and no system-scope fence, a PCIe round trip) is needed; the host polls the entry itself
       const unsigned long long entry = ((gstep + 1ull) << 32) | (unsigned long long)(unsigned)token;
@@ -253,6 +337,13 @@ __global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) 
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) {
+  sample_generic_body<false>(p, SampleProc{});
+}
+__global__ void __launch_bounds__(ST) sample_generic_proc_kernel(const SampleArgs p, const SampleProc q) {
+  sample_generic_body<true>(p, q);
 }
 
 
@@ -287,7 +378,8 @@ DTK_DEV int allreduce_sum_int(int v, Red2& r, int& ph) {
   return t;
 }
 
-__global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
+template <bool PROC>
+DTK_DEV void sample_body(const SampleArgs p, const SampleProc q) {
   __shared__ RedScratch red;
   __shared__ Red2 red2;
   __shared__ float sm_scan[32];
@@ -300,6 +392,16 @@ __global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
   const float T = sampling ? p.temperature : 1.f;
   unsigned long long gstep = p.gen_step ? *p.gen_step : 0ull;
   int ph = 0;
+  uint32_t *ban = nullptr, *pen = nullptr;
+  float penalty = 1.f, min_p = 0.f;
+  if constexpr (PROC) {
+    __shared__ uint32_t proc_masks[2 * (kProcMaxVocab / 32)];
+    ban = proc_masks;
+    pen = proc_masks + ((V + 31) >> 5);
+    build_proc_masks(q, b, sq.suppress, V, ban, pen);
+    penalty = q.tab->penalty;
+    min_p = q.tab->min_p;
+  }
 
   // 1. masks + temperature, running (max, argmax); entries beyond V are -inf (probability 0 everywhere below)
   float v[VPT];
@@ -311,6 +413,7 @@ __global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
     float x = -INFINITY;
     if (i < V) {
       x = __ldcg(lg + i);
+      if constexpr (PROC) x = apply_proc(x, i, penalty, ban, pen);
       if (i == p.bad_token || (sq.suppress && i == p.bs_token)) x = -INFINITY;
       x = x / T;
       if (x > mx) { mx = x; amx = i; }
@@ -369,10 +472,19 @@ __global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
     }
     // 5. renormalise over the nucleus; the final probability vector goes to the scratch row
     float z2 = 0.f;
+    if constexpr (PROC) {   // min-p: also drop p < min_p * p_max (p_max = invz is always kept)
+      const float mthr = min_p * invz;
 #pragma unroll
-    for (int j = 0; j < VPT; ++j) {
-      if (v[j] <= theta) v[j] = 0.f;
-      if (tid + j * ST < V) z2 += v[j];
+      for (int j = 0; j < VPT; ++j) {
+        if (v[j] <= theta || v[j] < mthr) v[j] = 0.f;
+        if (tid + j * ST < V) z2 += v[j];
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < VPT; ++j) {
+        if (v[j] <= theta) v[j] = 0.f;
+        if (tid + j * ST < V) z2 += v[j];
+      }
     }
     z2 = allreduce_sum(z2, red2, ph);
     const float invz2 = 1.f / z2;
@@ -443,6 +555,7 @@ __global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
     if (p.gen_tok) {
       p.gen_tok[b] = token;
       p.gen_pos[b] = min(p.gen_pos[b] + 1, p.max_pos);
+      if constexpr (PROC) append_hist(q, b, token);
       // ONE 8-byte store to the mapped pinned ring carries the token and its step stamp, so no ordering between two
       // host-visible stores (and no system-scope fence, a PCIe round trip) is needed; the host polls the entry itself
       const unsigned long long entry = ((gstep + 1ull) << 32) | (unsigned long long)(unsigned)token;
@@ -456,6 +569,9 @@ __global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) {
   }
 }
 
+__global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) { sample_body<false>(p, SampleProc{}); }
+__global__ void __launch_bounds__(ST) sample_proc_kernel(const SampleArgs p, const SampleProc q) { sample_body<true>(p, q); }
+
 }  // namespace
 
 static int g_sample_impl = 0;  // 0 = register-resident kernel when the vocabulary fits, 1 = always the generic kernel (tests)
@@ -466,6 +582,14 @@ cudaError_t launch_sample(const SampleArgs& a, cudaStream_t s, uint64_t* counter
   if (a.B <= 0 || a.B > 64) return cudaErrorInvalidValue;
   if (g_sample_impl == 0 && a.V <= ST * VPT) sample_kernel<<<a.B, ST, 0, s>>>(a);
   else sample_generic_kernel<<<a.B, ST, 0, s>>>(a);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sample_proc(const SampleArgs& a, const SampleProc& q, cudaStream_t s, uint64_t* counter) {
+  if (a.B <= 0 || a.B > 64 || a.V > kProcMaxVocab || !q.tab || !q.hist || !q.hist_len) return cudaErrorInvalidValue;
+  if (g_sample_impl == 0 && a.V <= ST * VPT) sample_proc_kernel<<<a.B, ST, 0, s>>>(a, q);
+  else sample_generic_proc_kernel<<<a.B, ST, 0, s>>>(a, q);
   if (counter) ++*counter;
   return cudaGetLastError();
 }

@@ -11,7 +11,7 @@ from typing import TYPE_CHECKING, Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import DtkConfig, DtkSampling, DtkWeightInfo
+from ._lib import DtkConfig, DtkProcessors, DtkSampling, DtkWeightInfo
 if TYPE_CHECKING:  # avoid a package-level import cycle (model/ imports this module)
     from .model.configuration import DetikzifyConfig
 
@@ -173,6 +173,34 @@ def random_arena_device(cfg: "DetikzifyConfig", device, seed: int = 0, ccfg: Opt
             k = vc.num_channels * vc.patch_size * vc.patch_size
             arena[info.offset // 2: info.offset // 2 + info.rows * info.cols].view(info.rows, info.cols)[:, k:] = 0
     return arena
+
+
+def _i32(xs: Sequence[int]):
+    xs = [int(x) for x in xs]
+    return (C.c_int32 * max(1, len(xs)))(*xs)
+
+
+def c_processors(repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_p: float = 0.0, eos_token_id: int = -1,
+                 ban_ids: Sequence[int] = (), begin_ids: Sequence[int] = (),
+                 words: Sequence[Sequence[int]] = ()) -> DtkProcessors:
+    """``dtk_processors`` (include/detikzify_b200.h): ``ban_ids`` always banned, ``begin_ids`` banned on rows whose suppress
+    flag is set, ``words`` bad-word sequences of two or more ids. The struct keeps its id arrays alive."""
+    words = [[int(i) for i in w] for w in words]
+    ban_ids, begin_ids = list(ban_ids), list(begin_ids)
+    ban, begin = _i32(ban_ids), _i32(begin_ids)
+    wid, wlen = _i32([i for w in words for i in w]), _i32([len(w) for w in words])
+    p = DtkProcessors(repetition_penalty=float(repetition_penalty), min_p=float(min_p),
+                      no_repeat_ngram_size=int(no_repeat_ngram_size), eos_token_id=int(eos_token_id),
+                      ban_ids=ban, n_ban=len(ban_ids), begin_ids=begin, n_begin=len(begin_ids),
+                      word_ids=wid, word_lens=wlen, n_words=len(words))
+    p._arrays = (ban, begin, wid, wlen)
+    return p
+
+
+def c_histories(histories: Sequence[Sequence[int]]):
+    """(concatenated ids, lengths) int32 arrays of per-row token histories."""
+    flat = [int(i) for h in histories for i in h]
+    return _i32(flat), _i32([len(h) for h in histories])
 
 
 class Engine:
@@ -428,6 +456,20 @@ class Engine:
         self._check(self.lib.dtk_sample(self._h, self._ptr(logits), B, C.byref(params), cs, ct, ci, self._ptr(out),
                                         self._ptr(probs), self._stream()), "dtk_sample")
         return out, probs
+
+    def set_processors(self, proc: Optional[dict], histories: Sequence[Sequence[int]] = (),
+                       eos_min_len: Optional[Sequence[int]] = None):
+        """HF logits processors for the following ``sample`` / ``gen_begin`` calls (``dtk_set_processors``); ``proc`` holds
+        ``c_processors`` keywords, None turns them off. ``histories[b]``: row b's ids so far (prompt + tokens, ending with
+        the first pending token before ``gen_begin``); ``eos_min_len[b]``: EOS is banned while the row is shorter."""
+        if proc is None:
+            self._check(self.lib.dtk_set_processors(self._h, None, 0, None, None, None, self._stream()), "dtk_set_processors")
+            return
+        B = len(histories)
+        cp = c_processors(**proc)
+        ids, lens = c_histories(histories)
+        eml = _i32(eos_min_len) if eos_min_len is not None else None
+        self._check(self.lib.dtk_set_processors(self._h, C.byref(cp), B, ids, lens, eml, self._stream()), "dtk_set_processors")
 
     # ------------------------------------------------------------------ fused generation loop
     def gen_begin(self, slots: Sequence[int], positions: Sequence[int], first_ids: Sequence[int], params: DtkSampling,

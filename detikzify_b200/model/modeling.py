@@ -8,6 +8,11 @@ reference drives at detikzify/infer/generate.py:218-227. What callers rely on:
   model.generate(input_ids=[1,T0], bad_words_ids=[[id]], begin_suppress_tokens=[id], pixel_values=...,
                  streamer=..., stopping_criteria=[...], temperature, top_p, top_k, max_length,
                  do_sample, **ignored) -> LongTensor [1,T]          (infer/generate.py:218-227)
+  HF's other logits processors, applied on the device in HF's order (``_processors``): repetition_penalty,
+  no_repeat_ngram_size, bad_words_ids (any number of entries of any length), min_length / min_new_tokens,
+  suppress_tokens, begin_suppress_tokens (a list), and min_p when sampling. Each falls back to the
+  ``generation_config`` attribute of the same name. Beam search, num_return_sequences, sequence_bias,
+  typical / epsilon / eta cutoffs and Python logits_processor callables are ignored.
   model.device / model.dtype / model.name_or_path / model.config.* / model.generation_config
   model.model.vision_model(pixel_values=...) -> .last_hidden_state, .pooler_output
                                                                (evaluate/imagesim.py:87,101-107)
@@ -105,6 +110,33 @@ class _Inner:
 
     def __init__(self, owner):
         self.vision_model = DetikzifyVisionModel(owner)
+
+
+class _Processors(SimpleNamespace):
+    """What a generate call's processor kwargs became: ``bad_token`` / ``bs_token`` for the sampler's single-id fields,
+    ``proc`` (``Engine.set_processors`` keywords, None when nothing beyond those two ids is asked for) and ``eos_min``
+    (EOS is banned while a sequence is shorter than ``eos_min(prompt_len)``)."""
+
+    def eos_min(self, prompt_len: int) -> int:
+        return prompt_len + self.min_new_tokens if self.min_new_tokens is not None else self.min_length
+
+
+def _id_list(name: str, value, V: int) -> List[int]:
+    vals = [value] if isinstance(value, int) else list(value)
+    out = []
+    for v in vals:
+        if isinstance(v, bool) or not isinstance(v, int) or not 0 <= v < V:
+            raise ValueError(f"`{name}` must hold token ids in [0, {V}), got {v!r}")
+        out.append(int(v))
+    return out
+
+
+def _int_arg(name: str, value) -> Optional[int]:
+    if value is None:
+        return None
+    if isinstance(value, bool) or not isinstance(value, int) or value < 0:
+        raise ValueError(f"`{name}` has to be a non-negative integer, but is {value!r}")
+    return int(value)
 
 
 class _KVSlot:
@@ -267,15 +299,49 @@ class DetikzifyForCausalLM:
             out.append(row.tolist())
         return out
 
-    @staticmethod
-    def _first(seq, default=-1) -> int:
-        try:
-            v = seq[0]
-            while isinstance(v, (list, tuple)):
-                v = v[0]
-            return int(v)
-        except (TypeError, IndexError):
-            return default
+    def _processors(self, bad_words_ids, begin_suppress_tokens, kw: Dict[str, Any], eos: int, sampling: bool) -> _Processors:
+        """The HF logits-processor kwargs of a generate call (HF generation/utils.py::_get_logits_processor), validated as HF
+        validates them, each falling back to the ``generation_config`` attribute of the same name. A call that asks for at
+        most one bad id and one begin-suppress id keeps the sampler's single-id fields (the reference's own call,
+        infer/generate.py:218-227); anything more runs the sampler's processor tables."""
+        gc, V = self.generation_config, self.config.vocab_size
+
+        def arg(name, value=None):
+            return getattr(gc, name, None) if value is None else value
+        penalty = arg("repetition_penalty", kw.get("repetition_penalty"))
+        if penalty is not None and (isinstance(penalty, bool) or not isinstance(penalty, (int, float)) or not penalty > 0):
+            raise ValueError(f"`repetition_penalty` has to be a strictly positive float, but is {penalty!r}")
+        ngram = _int_arg("no_repeat_ngram_size", arg("no_repeat_ngram_size", kw.get("no_repeat_ngram_size"))) or 0
+        min_length = _int_arg("min_length", arg("min_length", kw.get("min_length"))) or 0
+        min_new = _int_arg("min_new_tokens", arg("min_new_tokens", kw.get("min_new_tokens")))
+        min_p = arg("min_p", kw.get("min_p"))
+        if min_p is not None and (isinstance(min_p, bool) or not isinstance(min_p, (int, float)) or not 0 <= min_p <= 1):
+            raise ValueError(f"`min_p` has to be a float in [0, 1], but is {min_p!r}")
+        bad = arg("bad_words_ids", bad_words_ids)
+        words: List[List[int]] = []
+        if bad is not None:
+            if not isinstance(bad, (list, tuple)) or any(not isinstance(w, (list, tuple)) or not w for w in bad):
+                raise ValueError(f"`bad_words_ids` has to be a list of non-empty lists of token ids, but is {bad!r}")
+            words = [_id_list("bad_words_ids", w, V) for w in bad]
+            words = [w for w in words if w != [eos]]          # NoBadWordsLogitsProcessor drops [eos]
+        begin = arg("begin_suppress_tokens", begin_suppress_tokens)
+        begin = list(dict.fromkeys(_id_list("begin_suppress_tokens", begin, V))) if begin is not None else []
+        suppress = arg("suppress_tokens", kw.get("suppress_tokens"))
+        suppress = _id_list("suppress_tokens", suppress, V) if suppress is not None else []
+        singles = list(dict.fromkeys(w[0] for w in words if len(w) == 1))
+        multi = [w for w in words if len(w) > 1]
+        out = _Processors(min_length=min_length, min_new_tokens=min_new, bad_token=-1, bs_token=-1, proc=None)
+        active = ((penalty is not None and penalty != 1) or ngram > 0 or multi or len(singles) > 1 or suppress
+                  or len(begin) > 1 or min_length > 0 or (min_new is not None and min_new > 0)
+                  or (sampling and min_p is not None and min_p > 0))
+        if not active:
+            out.bad_token = singles[0] if singles else -1
+            out.bs_token = begin[0] if begin else -1
+            return out
+        out.proc = dict(repetition_penalty=float(penalty) if penalty is not None else 1.0, no_repeat_ngram_size=ngram,
+                        min_p=float(min_p) if (sampling and min_p is not None) else 0.0, eos_token_id=eos,
+                        ban_ids=singles + suppress, begin_ids=begin, words=multi)
+        return out
 
     # ---- prompt helpers shared by generate_batch / forward / score ----------------------------------
     def _image_span(self, ids_host: List[int]) -> Tuple[int, int]:
@@ -371,6 +437,8 @@ class DetikzifyForCausalLM:
         top_k = gc.top_k if top_k is None else top_k
         do_sample = gc.do_sample if do_sample is None else do_sample
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
+        procs = self._processors(bad_words_ids, begin_suppress_tokens, ignored, eos,
+                                 bool(do_sample) and float(temperature) >= 1e-5)
 
         ids2d = input_ids if input_ids.dim() == 2 else input_ids[None]
         if ids2d.shape[0] != 1:
@@ -420,9 +488,17 @@ class DetikzifyForCausalLM:
             self._call_counter += 1
             params = eng.sampling(
                 temperature=temperature, top_p=top_p, top_k=top_k or 0, do_sample=bool(do_sample),
-                bad_token=self._first(bad_words_ids), begin_suppress_token=self._first(begin_suppress_tokens),
+                bad_token=procs.bad_token, begin_suppress_token=procs.bs_token,
                 seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
-            first, _ = eng.sample(last_logits, params, suppress=[1], steps=[0])
+            eos_min = [procs.eos_min(T0)]
+            if procs.proc is not None:
+                eng.set_processors(procs.proc, [ids_host], eos_min)
+            try:
+                first, _ = eng.sample(last_logits, params, suppress=[1], steps=[0])
+            except BaseException:
+                if procs.proc is not None:
+                    eng.set_processors(None)
+                raise
             tok = int(first.item())
 
             out_buf = torch.empty(1, max_length, dtype=torch.int64)
@@ -441,6 +517,8 @@ class DetikzifyForCausalLM:
                     if tok == eos or len(new_tokens) >= n_new or criteria(cur, None):
                         break
                     if not started:
+                        if procs.proc is not None:   # the device history continues from prompt + the first new token
+                            eng.set_processors(procs.proc, [ids_host + new_tokens], eos_min)
                         eng.gen_begin([self._slot], [T0], [tok], params)
                         started = True
                     while launched < waited + 2 and launched < n_new - 1:
@@ -451,6 +529,8 @@ class DetikzifyForCausalLM:
             finally:
                 if started:
                     eng.gen_end()
+                if procs.proc is not None:
+                    eng.set_processors(None)
                 # decode step s wrote KV at T0+s for new_tokens[s]; only tokens the host has seen count
                 self._slot_tokens = list(ids_host) + new_tokens[: min(launched, len(new_tokens))]
             # exceptions escape before this point (the caller's error_callback feeds the streamer,
@@ -492,6 +572,8 @@ class DetikzifyForCausalLM:
         top_k = gc.top_k if top_k is None else top_k
         do_sample = gc.do_sample if do_sample is None else do_sample
         eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
+        procs = self._processors(bad_words_ids, begin_suppress_tokens, ignored, eos,
+                                 bool(do_sample) and float(temperature) >= 1e-5)
         prompts: List[List[int]] = [(p[0] if p.dim() == 2 else p).tolist() for p in input_ids]
         N = len(prompts)
         if N == 0:
@@ -519,6 +601,7 @@ class DetikzifyForCausalLM:
                     st.put(torch.tensor([prompts[i]], dtype=torch.int64))
             slots: List[int] = []
             base_slot = None
+            procs_set = False
             try:
                 for _ in range(N):
                     slots.append(eng.seq_alloc())
@@ -551,9 +634,13 @@ class DetikzifyForCausalLM:
                 self._call_counter += 1
                 params = eng.sampling(
                     temperature=temperature, top_p=top_p, top_k=top_k or 0, do_sample=bool(do_sample),
-                    bad_token=self._first(bad_words_ids), begin_suppress_token=self._first(begin_suppress_tokens),
+                    bad_token=procs.bad_token, begin_suppress_token=procs.bs_token,
                     seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
                 seq_ids = list(range(N))
+                eos_min = [procs.eos_min(len(p)) for p in prompts]
+                if procs.proc is not None:
+                    procs_set = True
+                    eng.set_processors(procs.proc, prompts, eos_min)
                 first, _ = eng.sample(torch.stack(last), params, suppress=[1] * N, steps=[0] * N, seq_ids=seq_ids)
                 toks = [int(t) for t in first.tolist()]
                 outs: List[List[int]] = [list(p) for p in prompts]
@@ -571,6 +658,8 @@ class DetikzifyForCausalLM:
                         accept(i, toks[i])
                 max_steps = max(lim - len(p) for p, lim in zip(prompts, limits)) - 1
                 if not all(done) and max_steps > 0:
+                    if procs.proc is not None:   # device histories continue from prompt + first token (at most max_len ids)
+                        eng.set_processors(procs.proc, [(p + [t])[:eng.max_len] for p, t in zip(prompts, toks)], eos_min)
                     eng.gen_begin(slots, [len(p) for p in prompts], toks, params, seq_ids)
                     launched = waited = 0
                     try:
@@ -592,6 +681,8 @@ class DetikzifyForCausalLM:
                 self._sync()
                 return result
             finally:
+                if procs_set:
+                    eng.set_processors(None)
                 for s in slots:
                     eng.seq_free(s)
                 if base_slot is not None:

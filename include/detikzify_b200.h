@@ -87,6 +87,29 @@ typedef struct dtk_sampling {
   uint64_t seed;
 } dtk_sampling;
 
+/* HF logits processors beyond one bad token and one begin-suppress token (HF generation/utils.py::_get_logits_processor,
+ * generation/logits_process.py), applied in HF's order before the temperature: repetition penalty
+ * (RepetitionPenaltyLogitsProcessor: x < 0 ? x * p : x / p in fp32 on every distinct id of the row's history), no-repeat
+ * n-gram (NoRepeatNGramLogitsProcessor), bad words (NoBadWordsLogitsProcessor: single ids always, a longer sequence bans
+ * its last id when the history ends with its other ids and is skipped when it is longer than the history), minimum length
+ * (MinLength / MinNewTokensLength: EOS banned while the history is shorter than the row's eos_min_len), suppress tokens
+ * (SuppressTokensLogitsProcessor) and begin-suppress tokens (SuppressTokensAtBeginLogitsProcessor: rows whose suppress
+ * flag is set); min-p (MinPLogitsWarper) after top-p when sampling. "Banned" = -inf, like dtk_sampling.bad_token.
+ * Limits: vocab <= 131072; n_ban + n_begin + n_words + 1 + (ids in word_ids) <= 4096. */
+typedef struct dtk_processors {
+  double repetition_penalty;  /* 1 -> off; > 0 */
+  double min_p;               /* 0 -> off; in [0, 1]; sampling only */
+  int32_t no_repeat_ngram_size; /* 0 -> off */
+  int32_t eos_token_id;       /* the id eos_min_len bans (-1 = none) */
+  const int32_t* ban_ids;     /* [n_ban] host: always banned (bad words of length 1, suppress_tokens) */
+  int32_t n_ban;
+  const int32_t* begin_ids;   /* [n_begin] host: banned on rows whose suppress flag is set */
+  int32_t n_begin;
+  const int32_t* word_ids;    /* host: bad-word sequences of length >= 2, concatenated */
+  const int32_t* word_lens;   /* [n_words] host: their lengths */
+  int32_t n_words;
+} dtk_processors;
+
 typedef struct dtk_engine dtk_engine;
 
 DTK_API int dtk_abi_version(void);
@@ -207,6 +230,17 @@ DTK_API int dtk_sample(dtk_engine* eng, const float* logits, int B, const dtk_sa
                const int* suppress, const uint32_t* steps, const uint32_t* seq_ids,
                int64_t* out_ids, float* probs_out, void* stream);
 
+/* ---- logits processors (dtk_processors) for the following dtk_sample and dtk_gen_begin calls, until a call with
+ *      proc == NULL turns them off. Replaces the HF processors listed at dtk_processors for B rows: row b's history is
+ *      hist_len[b] ids (prompt + tokens so far, HF's input_ids) taken in order from the concatenated host array hist_ids,
+ *      at most max_len each; eos_min_len host int[B] (may be NULL = 0): EOS is banned while the row's history is shorter.
+ *      The histories live in the engine; the generation loop appends every token it draws (clamped at max_len), so
+ *      before dtk_gen_begin they must end with first_ids. dtk_sample and dtk_gen_begin then take B <= the rows given
+ *      here, and greedy batch-1 generation takes its token from the sampler instead of the persistent kernel's fused
+ *      argmax. Not allowed inside a generation loop. Synchronises `stream`. ----------------------------------------- */
+DTK_API int dtk_set_processors(dtk_engine* eng, const dtk_processors* proc, int B, const int32_t* hist_ids,
+                               const int32_t* hist_len, const int32_t* eos_min_len, void* stream);
+
 /* ---- fused generation loop state (device-resident; one graph launch per token).
  *      dtk_gen_begin: bind B slots whose prompts are prefilled to `positions[b]` tokens and
  *      whose first pending token is first_ids[b] (already sampled from the prefill logits).
@@ -280,6 +314,12 @@ DTK_API int dtk_dbg_lm_logprob(const void* A_bf16, const void* W_bf16, int M, in
 DTK_API int dtk_dbg_sample(const float* logits, int B, int V, const dtk_sampling* params, const int* suppress,
                            const uint32_t* steps, const uint32_t* seq_ids, int impl, int64_t* out_ids, float* probs,
                            void* stream);
+/* dtk_dbg_sample with logits processors (dtk_set_processors' arguments for B rows of at most max_len ids); the engine's
+ * processor sampler without an engine; synchronises `stream` */
+DTK_API int dtk_dbg_sample_proc(const float* logits, int B, int V, const dtk_sampling* params, const int* suppress,
+                                const uint32_t* steps, const uint32_t* seq_ids, int impl, const dtk_processors* proc,
+                                const int32_t* hist_ids, const int32_t* hist_len, const int32_t* eos_min_len, int max_len,
+                                int64_t* out_ids, float* probs, void* stream);
 /* q,k,v,o bf16 [B, T, heads, head_dim]; head_dim in {72,128} */
 DTK_API int dtk_dbg_flash_attn(const void* q, const void* k, const void* v, void* o, int B,
                                int heads, int Tq, int Tk, int head_dim, int causal, int q_pos0,
