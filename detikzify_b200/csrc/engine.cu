@@ -1991,6 +1991,32 @@ int dtk_dbg_pack_bytes(dtk_engine* eng, int64_t offset, int64_t nbytes, void* ou
   return DTK_OK;
 }
 
+int dtk_dbg_kv_read(dtk_engine* eng, int slot, int layer, int pos0, int n, void* k_out, void* v_out, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(k_out && v_out, "null pointer");
+  DTK_REQUIRE(slot >= 0 && slot < c.max_seqs && eng->slot_used[slot], "slot is not allocated");
+  DTK_REQUIRE(layer >= 0 && layer < c.layers, "layer");
+  DTK_REQUIRE(pos0 >= 0 && n >= 0 && (int64_t)pos0 + n <= c.max_len, "positions outside [0, max_len)");
+  DTK_CK(cudaSetDevice(eng->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t HD = c.head_dim;
+  const size_t src_pitch = (size_t)c.max_len * HD * sizeof(bf16), dst_pitch = (size_t)n * HD * sizeof(bf16);
+  // positions below the slot's shared length resolve to the lending slot, as the decode attention kernels read them
+  const int split = std::min(std::max(eng->share_len[slot], pos0), pos0 + n);
+  const int parts[2][3] = {{eng->share_base[slot] >= 0 ? eng->share_base[slot] : slot, pos0, split}, {slot, split, pos0 + n}};
+  for (const auto& pt : parts) {
+    if (pt[2] <= pt[1]) continue;
+    const bf16* k = kv_layer(eng, pt[0], layer) + (int64_t)pt[1] * HD;
+    const size_t off = (size_t)(pt[1] - pos0) * HD, width = (size_t)(pt[2] - pt[1]) * HD * sizeof(bf16);
+    DTK_CK(cudaMemcpy2DAsync(static_cast<bf16*>(k_out) + off, dst_pitch, k, src_pitch, width, c.kv_heads,
+                             cudaMemcpyDeviceToDevice, s));
+    DTK_CK(cudaMemcpy2DAsync(static_cast<bf16*>(v_out) + off, dst_pitch, k + eng->kv_v_offset, src_pitch, width, c.kv_heads,
+                             cudaMemcpyDeviceToDevice, s));
+  }
+  return DTK_OK;
+}
+
 int dtk_dbg_gemm_impl(int impl) {
   if (impl >= 0) {
     set_gemm_impl(impl & 0xff);

@@ -292,6 +292,10 @@ DTK_API int dtk_dbg_mega_trace(dtk_engine* eng, long long* out_host, int max_val
 /* bytes [offset, offset + nbytes) of the packed decode tiles (option "decode_pack" = 1): [layer][wqkv | wo | wgu | wd tiles],
  * then the lm_head tiles, 6688 bytes per tile (launch.h, MegaPack) */
 DTK_API int dtk_dbg_pack_bytes(dtk_engine* eng, int64_t offset, int64_t nbytes, void* out_host);
+/* copy (stream-ordered, no engine state changes) the cached bf16 keys and values of positions [pos0, pos0 + n) of one layer
+ * of an allocated slot into k_out / v_out, each [kv_heads][n][head_dim]. Positions below the slot's shared length come from
+ * the slot that lends them, as decode reads them. DTK_ERR_INVALID: slot not allocated, layer or range outside the cache. */
+DTK_API int dtk_dbg_kv_read(dtk_engine* eng, int slot, int layer, int pos0, int n, void* k_out, void* v_out, void* stream);
 /* select the dense GEMM implementation used by dtk_dbg_gemm and the engines of this process:
  * 0 = mma.sync, 1 = wgmma one 128 x 128 tile per CTA, 2 (default) = persistent 128 x 256 wgmma kernel,
  * -1 = query only; returns the current setting. Bits 8..11 of a
