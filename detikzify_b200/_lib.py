@@ -90,6 +90,9 @@ SYMBOLS = {
     "dtk_gen_step": (C.c_int, [_P, _P]),
     "dtk_gen_wait": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_int32)]),
     "dtk_gen_end": (C.c_int, [_P]),
+    "dtk_gen_admit": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_uint32, C.POINTER(C.c_int32), C.c_int, C.c_int, _P]),
+    "dtk_gen_retire": (C.c_int, [_P, C.c_int, _P]),
+    "dtk_gen_first": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int32)]),
     "dtk_set_option": (C.c_int, [_P, C.c_char_p, C.c_int64]),
     "dtk_get_option": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_int64)]),
     "dtk_decode_bytes": (C.c_uint64, [C.POINTER(DtkConfig), C.c_int]),

@@ -101,10 +101,11 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const GemvArgs p) {
         o[r0] += a0; o[r1] += a1;
       } else if (MODE == GEMV_GLU) {
         p.out[(int64_t)b * p.out_stride + item] = silu(a0) * a1;
-      } else {  // GEMV_QKV: rotate-half RoPE on q/k, write k/v straight into the slot cache
+      } else {  // GEMV_QKV: rotate-half RoPE on q/k, write k/v straight into the slot cache (not for a retired row)
         const int pos = p.pos[b], slot = p.slots[b];
         const int i = r0 & (HD - 1);  // < HD / 2
-        if (r0 < p.q_dim + p.kv_dim) {
+        if (r0 >= p.q_dim && p.active && !p.active[b]) {
+        } else if (r0 < p.q_dim + p.kv_dim) {
           const float2 cs = *reinterpret_cast<const float2*>(p.rope_cs + ((int64_t)pos * (HD / 2) + i) * 2);
           const float y0 = a0 * cs.x - a1 * cs.y, y1 = a1 * cs.x + a0 * cs.y;
           if (r0 < p.q_dim) {
@@ -159,9 +160,12 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(const DecodeAtt
   const int tid = threadIdx.x, hw = tid / LPK, l16 = tid & (LPK - 1);
   const int T = p.pos[b] + 1, slot = p.slots[b];
   const int kvh = head / p.kv_group;
+  // a retired row of a generation loop reads no keys (its slot may already belong to another sequence); its CTAs still
+  // take part in the counters protocol and its output is zero
+  const bool live = !p.active || p.active[b];
   int chunk = (T - p.key_begin + p.nsplit - 1) / p.nsplit;   // key_begin > 0: the shared prefix was reduced by the prefix kernel
   chunk = (chunk + 7) & ~7;
-  const int j0 = p.key_begin + split * chunk, j1 = min(T, j0 + chunk);
+  const int j0 = p.key_begin + split * chunk, j1 = live ? min(T, j0 + chunk) : j0;
   const bf16* kb = p.kv_base + (int64_t)slot * p.kv_slot_stride + (int64_t)kvh * p.max_len * HD;
   const bf16* vb = kb + p.kv_v_offset;
   // shared prefix: positions below shlen live in another slot (one copy for all rollouts of a figure)
@@ -257,7 +261,7 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(const DecodeAtt
       L += __ldcg(p.part_ml + (base + s) * 2 + 1) * w;
       O += __ldcg(p.part_o + (base + s) * HD + d) * w;
     }
-    const float res = O / L;
+    const float res = live ? O / L : 0.f;
     p.out[(int64_t)b * p.out_stride + head * HD + d] = res;
     if (p.out_bf16) p.out_bf16[(int64_t)b * p.out_stride + head * HD + d] = __float2bfloat16_rn(res);
     if (tid == 0) p.counters[b * p.heads + head] = 0u;

@@ -211,6 +211,10 @@ struct dtk_engine {
   float *d_part_o = nullptr, *d_part_ml = nullptr;
   unsigned int* d_counters = nullptr;  // [max_batch*heads] + 1 (sampler done counter)
   int *d_slots = nullptr, *d_pos = nullptr, *d_tok = nullptr, *d_share_slot = nullptr, *d_share_len = nullptr;
+  // per-row loop state the batched step and its sampler read: activity (a retired row writes no KV and draws nothing), RNG
+  // counter base (a row admitted at step s0 draws counter 1 + step - s0) and RNG stream
+  int* d_active = nullptr;
+  uint32_t *d_row_step = nullptr, *d_row_seq = nullptr;
   unsigned long long* d_gen = nullptr;  // [0] = step counter
   // ViT workspace (grows with batch)
   int vit_cap = 0;
@@ -230,7 +234,13 @@ struct dtk_engine {
   int gen_B = 0;
   dtk_sampling gen_params{};
   unsigned long long* host_ring = nullptr;   // pinned, mapped: [ring][64] entries ((step + 1) << 32) | token
-  unsigned long long* dev_ring = nullptr;
+  unsigned long long* dev_ring = nullptr;     // ... followed by the admission mailbox [64]: (stamp << 32) | first token
+  // admissions (dtk_gen_admit): host mirror of d_active, per-row admission stamps, and a pinned staging row per loop row for
+  // the admitted history (reused only after the event of the row's previous admission has passed)
+  std::vector<char> row_active;
+  std::vector<uint32_t> admit_stamp;
+  int* h_admit_hist = nullptr;
+  std::vector<cudaEvent_t> admit_ev;
   int ring = 256;
   std::map<std::string, cudaGraphExec_t> graphs;
   cudaGraphExec_t gen_graph = nullptr;
@@ -328,16 +338,23 @@ struct StateArgs {
   int n;
   int slots[64], pos[64], share_slot[64], share_len[64];
   long long tok[64];
-  int have_tok;
+  uint32_t seq[64];
+  int have_tok;   // dtk_gen_begin: also the first tokens, RNG streams seq[i] and counter base 1
 };
-__global__ void set_state_kernel(StateArgs a, int* slots, int* pos, int* tok, int* share_slot, int* share_len) {
+__global__ void set_state_kernel(StateArgs a, int* slots, int* pos, int* tok, int* share_slot, int* share_len, int* active,
+                                 uint32_t* row_step, uint32_t* row_seq) {
   int i = threadIdx.x;
   if (i < a.n) {
     slots[i] = a.slots[i];
     pos[i] = a.pos[i];
     share_slot[i] = a.share_slot[i];
     share_len[i] = a.share_len[i];
-    if (a.have_tok) tok[i] = (int)a.tok[i];
+    active[i] = 1;
+    if (a.have_tok) {
+      tok[i] = (int)a.tok[i];
+      row_step[i] = 1u;
+      row_seq[i] = a.seq[i];
+    }
   }
 }
 // rows of a batched step that all borrow the same prefix [0, len) from the same slot (the rollouts of one figure)
@@ -832,7 +849,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
     for (int l = 0; l < c.layers; ++l) {
       DTK_CK(launch_rmsnorm(eng->d_x, H, W(eng, LN("dec.L", l, "norm1")), c.rms_eps, B, H, eng->p_xn, s, lc));
       DTK_CK(gemm(eng->p_xn, H, W(eng, LN("dec.L", l, "wqkv")), qkvd, nullptr, 0, eng->p_qkv, nullptr, qkvd, l, 0));
-      DTK_CK(launch_rope_kv_decode(eng->p_qkv, B, eng->d_slots, eng->d_pos, c.heads, c.kv_heads, eng->rope_cs, eng->d_q,
+      DTK_CK(launch_rope_kv_decode(eng->p_qkv, B, eng->d_slots, eng->d_pos, eng->d_active, c.heads, c.kv_heads, eng->rope_cs, eng->d_q,
                                    kv_layer(eng, 0, l), eng->kv_slot_stride, eng->kv_v_offset, c.max_len, HD, s, lc, cas ? eng->p_q : nullptr));
       if (cas) {
         AttnArgs f{};
@@ -853,6 +870,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
         a.head_dim = HD; a.scale = scale;
         a.part_o = eng->d_part_o; a.part_ml = eng->d_part_ml; a.counters = eng->d_counters;
         a.out = eng->d_att; a.out_stride = qd; a.out_bf16 = eng->p_att;   // bf16 copy = the o-proj operand (no cast launch)
+        a.active = eng->d_active;
         if (cas) { a.key_begin = eng->cas_len; a.np = nsplit + csplit; }
         DTK_CK(launch_decode_attn(a, s, lc));
       }
@@ -873,7 +891,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
       g.out = eng->d_q; g.out_stride = qd; g.B = B;
       g.slots = eng->d_slots; g.pos = eng->d_pos; g.rope_cs = eng->rope_cs;
       g.kv_base = kv_layer(eng, 0, l); g.kv_slot_stride = eng->kv_slot_stride; g.kv_v_offset = eng->kv_v_offset;
-      g.q_dim = qd; g.kv_dim = kd; g.max_len = c.max_len; g.head_dim = HD;
+      g.q_dim = qd; g.kv_dim = kd; g.max_len = c.max_len; g.head_dim = HD; g.active = eng->d_active;
       DTK_CK(launch_gemv(g, s, lc));
     }
     {
@@ -883,7 +901,7 @@ int decode_launches(dtk_engine* eng, int B, const int64_t* tok64, float* logits,
       a.B = B; a.heads = c.heads; a.kv_group = c.heads / c.kv_heads; a.max_len = c.max_len; a.nsplit = nsplit;
       a.head_dim = HD; a.scale = scale;
       a.part_o = eng->d_part_o; a.part_ml = eng->d_part_ml; a.counters = eng->d_counters;
-      a.out = eng->d_att; a.out_stride = qd;
+      a.out = eng->d_att; a.out_stride = qd; a.active = eng->d_active;
       DTK_CK(launch_decode_attn(a, s, lc));
     }
     {
@@ -1081,6 +1099,9 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
   DTK_ALLOC(eng->d_tok, MB);
   DTK_ALLOC(eng->d_share_slot, MB);
   DTK_ALLOC(eng->d_share_len, MB);
+  DTK_ALLOC(eng->d_active, MB);
+  DTK_ALLOC(eng->d_row_step, MB);
+  DTK_ALLOC(eng->d_row_seq, MB);
   DTK_CK(cudaMemset(eng->d_share_slot, 0, MB * sizeof(int)));
   DTK_CK(cudaMemset(eng->d_share_len, 0, MB * sizeof(int)));
   DTK_ALLOC(eng->d_gen, 2);
@@ -1146,8 +1167,8 @@ int dtk_create(const dtk_config* cfg, const void* weight_arena, uint64_t arena_b
       eng->mega_ok = true;
     }
   }
-  DTK_CK(cudaHostAlloc((void**)&eng->host_ring, (size_t)eng->ring * 64 * sizeof(unsigned long long), cudaHostAllocMapped));
-  std::memset(eng->host_ring, 0, (size_t)eng->ring * 64 * sizeof(unsigned long long));
+  DTK_CK(cudaHostAlloc((void**)&eng->host_ring, (size_t)(eng->ring + 1) * 64 * sizeof(unsigned long long), cudaHostAllocMapped));
+  std::memset(eng->host_ring, 0, (size_t)(eng->ring + 1) * 64 * sizeof(unsigned long long));
   DTK_CK(cudaHostGetDevicePointer((void**)&eng->dev_ring, eng->host_ring, 0));
   DTK_CK(cudaDeviceSynchronize());
   return DTK_OK;
@@ -1163,11 +1184,13 @@ int dtk_destroy(dtk_engine* eng) {
                   eng->d_att, eng->d_h, eng->d_logits, eng->d_scratch, eng->d_part_o, eng->d_part_ml, eng->d_counters,
                   eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_gen, eng->d_amax, eng->d_bar, eng->d_dbg, eng->d_dbg2, eng->d_head_cnt, eng->d_tiled, eng->d_tiled_lm, eng->d_tiled8, eng->d_tiledpk, eng->d_pk_esc, eng->d_tagged, eng->v_x, eng->v_small_f, eng->v_pq, eng->v_xn,
                   eng->v_qkv, eng->v_att, eng->v_h, eng->v_small_b, eng->lse_part, eng->lse_tgt, eng->d_proc_tab, eng->d_hist,
-                  eng->d_hist_len};
+                  eng->d_hist_len, eng->d_active, eng->d_row_step, eng->d_row_seq};
   for (void* p : ptrs) if (p) cudaFree(p);
   dtk_adapter_detach(eng);
   if (eng->cap_stream) cudaStreamDestroy(eng->cap_stream);
   if (eng->host_ring) cudaFreeHost(eng->host_ring);
+  if (eng->h_admit_hist) cudaFreeHost(eng->h_admit_hist);
+  for (cudaEvent_t e : eng->admit_ev) cudaEventDestroy(e);
   cudaGetLastError();
   delete eng;
   return DTK_OK;
@@ -1642,7 +1665,8 @@ int dtk_decode(dtk_engine* eng, const int* slots, const int* positions, const in
   }
   DTK_CK(cudaSetDevice(eng->device));
   cudaStream_t s = (cudaStream_t)stream;
-  set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len);
+  set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_active,
+                                    eng->d_row_step, eng->d_row_seq);
   ++eng->launches;
   DTK_CK(cudaGetLastError());
   set_cascade(eng, st);
@@ -1721,25 +1745,29 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
     DTK_REQUIRE(slots[i] >= 0 && slots[i] < c.max_seqs, "slot");
     DTK_REQUIRE(positions[i] >= 0 && positions[i] < c.max_len, "position exceeds max_len");
     DTK_REQUIRE(positions[i] >= eng->share_len[slots[i]] && positions[i] >= eng->shared_upto[slots[i]], "position lies inside a shared prefix");
-    st.slots[i] = slots[i]; st.pos[i] = positions[i]; st.tok[i] = first_ids_host[i];
+    st.slots[i] = slots[i]; st.pos[i] = positions[i]; st.tok[i] = first_ids_host[i]; st.seq[i] = seq_ids ? seq_ids[i] : (uint32_t)i;
     st.share_slot[i] = eng->share_base[slots[i]] >= 0 ? eng->share_base[slots[i]] : slots[i];
     st.share_len[i] = eng->share_len[slots[i]];
   }
   set_cascade(eng, st);
-  set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len);
+  set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_active,
+                                    eng->d_row_step, eng->d_row_seq);
   reset_gen_kernel<<<1, 1, 0, s>>>(eng->d_gen, eng->d_counters + (int64_t)c.max_batch * c.heads, params->seed);
   eng->launches += 2;
   DTK_CK(cudaGetLastError());
   DTK_CK(cudaStreamSynchronize(s));
-  std::memset(eng->host_ring, 0, (size_t)eng->ring * 64 * sizeof(unsigned long long));  // stamps restart at step 1
+  std::memset(eng->host_ring, 0, (size_t)(eng->ring + 1) * 64 * sizeof(unsigned long long));  // stamps restart at step 1
+  eng->row_active.assign(64, 0);
+  std::fill(eng->row_active.begin(), eng->row_active.begin() + B, 1);
+  eng->admit_stamp.assign(64, 0u);
 
   eng->gen_B = B;
   eng->gen_params = *params;
   eng->gen_stream = s;
-  {  // sampler arguments of the loop (suppress = 0, RNG counter = 1 + step)
+  {  // sampler arguments of the loop (suppress = 0; RNG counter row_step + step on stream row_seq, set above to 1 and seq_ids)
     SampleArgs& a = eng->gen_sample;
     fill_sample_args(eng, a, eng->d_logits, B, *params);
-    for (int i = 0; i < B; ++i) { a.seq[i].suppress = 0; a.seq[i].step = 1; a.seq[i].seq_id = seq_ids ? seq_ids[i] : (uint32_t)i; }
+    a.active = eng->d_active; a.row_step = eng->d_row_step; a.row_seq = eng->d_row_seq;
     a.gen_tok = eng->d_tok; a.gen_pos = eng->d_pos; a.gen_step = eng->d_gen; a.seed_dev = eng->d_gen + 1; a.seed = 0;
     a.host_ring = eng->dev_ring; a.ring = eng->ring;
     a.done_counter = eng->d_counters + (int64_t)c.max_batch * c.heads;
@@ -1761,7 +1789,6 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
   skey += "|g" + std::to_string(eng->decode_gemm_min_batch) + "|i" + std::to_string(get_gemm_impl());
   skey += "|c" + std::to_string(eng->cas_slot) + ":" + std::to_string(eng->cas_len);   // shared-prefix attention bakes slot and length in
   if (eng->gen_proc) skey += "|P";   // processor tables and histories are read from engine buffers at replay
-  if (seq_ids) for (int i = 0; i < B; ++i) skey += "," + std::to_string(seq_ids[i]);
   auto it = eng->graphs.find(skey);
   if (it == eng->graphs.end()) {
     cudaGraph_t graph = nullptr;
@@ -1840,6 +1867,108 @@ int dtk_gen_wait(dtk_engine* eng, int64_t step, int32_t* tokens_out_host) {
     }
     tokens_out_host[i] = (int32_t)(uint32_t)(e & 0xffffffffull);
   }
+  return DTK_OK;
+}
+
+int dtk_gen_admit(dtk_engine* eng, int row, int slot, int position, const float* logits, uint32_t seq_id,
+                  const int32_t* hist_ids, int hist_len, int eos_min_len, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(eng->gen_B > 0, "dtk_gen_begin not called");
+  if (eng->gen_mega) {
+    eng->err = "unsupported: the batch-1 persistent generation loop takes no admissions";
+    return DTK_ERR_UNSUPPORTED;
+  }
+  DTK_REQUIRE((cudaStream_t)stream == eng->gen_stream, "admissions are enqueued on the loop's stream");
+  DTK_REQUIRE(row >= 0 && row < eng->gen_B, "row outside the loop's rows");
+  DTK_REQUIRE(!eng->row_active[row], "row is active (dtk_gen_retire it first)");
+  DTK_REQUIRE(slot >= 0 && slot < c.max_seqs && eng->slot_used[slot], "slot is not allocated");
+  DTK_REQUIRE(position >= 0 && position < c.max_len, "position exceeds max_len");
+  DTK_REQUIRE(position >= eng->share_len[slot] && position >= eng->shared_upto[slot], "position lies inside a shared prefix");
+  DTK_REQUIRE(logits, "null logits");
+  const int share_slot = eng->share_base[slot] >= 0 ? eng->share_base[slot] : slot, share_len = eng->share_len[slot];
+  // the shared-prefix attention of this loop's graph reads one baked prefix for every row
+  DTK_REQUIRE(eng->cas_len == 0 || (share_slot == eng->cas_slot && share_len == eng->cas_len),
+              "the loop runs shared-prefix (cascade) attention over another prefix than the slot borrows");
+  if (eng->gen_proc) {
+    DTK_REQUIRE(hist_len > 0 && hist_len <= c.max_len && hist_ids, "processors need the row's history (the prompt)");
+    for (int i = 0; i < hist_len; ++i) DTK_REQUIRE(hist_ids[i] >= 0 && hist_ids[i] < c.vocab, "history id outside [0, vocab)");
+  }
+  DTK_CK(cudaSetDevice(eng->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  SampleArgs a = eng->gen_sample;   // the loop's parameters, without its state: counter 0 on the request's stream
+  a.gen_tok = nullptr; a.gen_pos = nullptr; a.gen_step = nullptr; a.host_ring = nullptr; a.done_counter = nullptr;
+  a.active = nullptr; a.row_step = nullptr; a.row_seq = nullptr; a.out_ids = nullptr;
+  a.seq[row].suppress = 1; a.seq[row].step = 0; a.seq[row].seq_id = seq_id;
+  SampleAdmit m{};
+  m.logits = logits; m.row = row; m.slot = slot; m.pos = position; m.share_slot = share_slot; m.share_len = share_len;
+  m.hist_len = hist_len; m.eos_min = eos_min_len; m.seq_id = seq_id; m.stamp = ++eng->admit_stamp[row];
+  m.slots = eng->d_slots; m.posv = eng->d_pos; m.tok = eng->d_tok; m.share_slots = eng->d_share_slot;
+  m.share_lens = eng->d_share_len; m.active = eng->d_active; m.row_step = eng->d_row_step; m.row_seq = eng->d_row_seq;
+  m.gen_step = eng->d_gen; m.tab = eng->d_proc_tab; m.mailbox = eng->dev_ring + (size_t)eng->ring * 64;
+  SampleProc q{};
+  if (eng->gen_proc) {
+    if (!eng->h_admit_hist) {
+      DTK_CK(cudaHostAlloc((void**)&eng->h_admit_hist, (size_t)c.max_batch * c.max_len * sizeof(int), cudaHostAllocDefault));
+      eng->admit_ev.assign(c.max_batch, nullptr);
+      for (auto& e : eng->admit_ev) DTK_CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    // the row's staging buffer was last read by its previous admission's copy, which ran before that request's first
+    // step: in a loop that waits for its steps this event has long passed
+    DTK_CK(cudaEventSynchronize(eng->admit_ev[row]));
+    int* stage = eng->h_admit_hist + (size_t)row * c.max_len;
+    std::memcpy(stage, hist_ids, (size_t)hist_len * sizeof(int));
+    DTK_CK(cudaMemcpyAsync(eng->d_hist + (size_t)row * c.max_len, stage, (size_t)hist_len * sizeof(int), cudaMemcpyHostToDevice, s));
+    DTK_CK(cudaEventRecord(eng->admit_ev[row], s));
+    q = proc_args(eng);
+  }
+  DTK_CK(launch_sample_admit(a, eng->gen_proc ? &q : nullptr, m, s, &eng->launches));
+  eng->row_active[row] = 1;
+  return DTK_OK;
+}
+
+int dtk_gen_retire(dtk_engine* eng, int row, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->gen_B > 0, "dtk_gen_begin not called");
+  if (eng->gen_mega) {
+    eng->err = "unsupported: the batch-1 persistent generation loop has no row activity";
+    return DTK_ERR_UNSUPPORTED;
+  }
+  DTK_REQUIRE((cudaStream_t)stream == eng->gen_stream, "retirements are enqueued on the loop's stream");
+  DTK_REQUIRE(row >= 0 && row < eng->gen_B, "row outside the loop's rows");
+  DTK_CK(cudaSetDevice(eng->device));
+  DTK_CK(cudaMemsetAsync(eng->d_active + row, 0, sizeof(int), (cudaStream_t)stream));
+  eng->row_active[row] = 0;
+  return DTK_OK;
+}
+
+int dtk_gen_first(dtk_engine* eng, int row, int32_t* token_out_host) {
+  if (!eng) return DTK_ERR_INVALID;
+  DTK_REQUIRE(eng->gen_B > 0 && token_out_host, "gen state/out");
+  DTK_REQUIRE(row >= 0 && row < eng->gen_B && eng->admit_stamp[row] > 0, "row was not admitted in this loop");
+  volatile const unsigned long long* box = eng->host_ring + (size_t)eng->ring * 64 + row;
+  const unsigned long long want = eng->admit_stamp[row];
+  auto t0 = std::chrono::steady_clock::now();
+  uint64_t spins = 0;
+  unsigned long long e;
+  while (((e = *box) >> 32) != want) {
+    if ((++spins & 0x3ff) == 0) {
+      cudaError_t q = cudaStreamQuery(eng->gen_stream);
+      if (q != cudaSuccess && q != cudaErrorNotReady) {
+        eng->err = std::string("stream error while waiting for an admitted row's first token: ") + cudaGetErrorString(q);
+        return DTK_ERR_CUDA;
+      }
+      if (q == cudaSuccess && (*box >> 32) != want) {
+        eng->err = "stream idle but the admission never published its first token";
+        return DTK_ERR_INVALID;
+      }
+      if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(60)) {
+        eng->err = "timeout waiting for an admitted row's first token";
+        return DTK_ERR_CUDA;
+      }
+    }
+  }
+  *token_out_host = (int32_t)(uint32_t)(e & 0xffffffffull);
   return DTK_OK;
 }
 
@@ -1944,6 +2073,7 @@ int dtk_get_option(dtk_engine* eng, const char* key, int64_t* value) {
   if (std::strcmp(key, "decode_persistent") == 0) { *value = (eng->decode_impl == 1 && eng->mega_ok) ? 1 : 0; return DTK_OK; }
   if (std::strcmp(key, "gemm_impl") == 0) { *value = get_gemm_impl(); return DTK_OK; }
   if (std::strcmp(key, "decode_gemm_min_batch") == 0) { *value = eng->decode_gemm_min_batch; return DTK_OK; }
+  if (std::strcmp(key, "cascade_attn") == 0) { *value = eng->cascade_attn; return DTK_OK; }
   if (std::strcmp(key, "sample_impl") == 0) { *value = get_sample_impl(); return DTK_OK; }
   if (std::strcmp(key, "mega_flags") == 0) { *value = eng->mega_flags; return DTK_OK; }
   if (std::strcmp(key, "mega_debug") == 0) { *value = eng->mega_debug; return DTK_OK; }

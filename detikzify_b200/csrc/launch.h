@@ -123,7 +123,8 @@ cudaError_t launch_embed_splice(const int64_t* ids, int T, int start_pos, const 
                                 cudaStream_t s, uint64_t* counter);
 // decoder RoPE + KV append, head_dim hd in {64, 128}; rope_cs fp32 [max_len, hd/2, 2]; cache rows [kv_head][max_len][hd].
 // decode: qkv fp32 [B, qd+2kd] -> roped q fp32 (and optionally bf16) [B, qd]; K/V of row b into slot slots[b] at pos[b]
-cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, int heads, int kv_heads,
+// unless active[b] == 0 (a retired row of a generation loop, whose slot may already hold another sequence)
+cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, const int* active, int heads, int kv_heads,
                                   const float* rope_cs, float* q_out, bf16* kv_base, int64_t kv_slot_stride,
                                   int64_t kv_v_offset, int max_len, int hd, cudaStream_t s, uint64_t* counter, bf16* q_bf16 = nullptr);
 // prefill: qkv fp32 [T, qd+2kd] -> roped q bf16 [T, qd]; K/V bf16 into the cache at positions start_pos+t
@@ -161,6 +162,7 @@ struct GemvArgs {
   int64_t kv_v_offset;        // elements from K to V of the same layer
   int q_dim, kv_dim, max_len;
   int head_dim;               // 64 or 128
+  const int* active;          // device int[B] or null: rows with active[b] == 0 append no K/V
 };
 cudaError_t launch_gemv(const GemvArgs& a, cudaStream_t s, uint64_t* counter);
 
@@ -189,6 +191,7 @@ struct DecodeAttnArgs {
   // partial slots [nsplit, np); this kernel covers [key_begin, pos] and its merge adds all np partials. 0 / nsplit = off.
   int key_begin, np;
   bf16* out_bf16;             // optional bf16 copy of the output (the o-proj GEMM operand), same layout
+  const int* active;          // device int[B] or null: a row with active[b] == 0 reads no keys and gets a zero output
 };
 cudaError_t launch_decode_attn(const DecodeAttnArgs& a, cudaStream_t s, uint64_t* counter);
 
@@ -218,6 +221,12 @@ struct SampleArgs {
   int ring;
   int max_pos;                    // gen_pos is clamped to this (max_len - 1)
   unsigned int* done_counter;     // device, zero-initialised, self-resetting
+  // generation loop with admissions (device [B], all optional): a row with active[b] == 0 draws nothing, publishes the
+  // sentinel token -1 with its step stamp and still counts in done_counter (gen_tok, gen_pos and its history stay as they
+  // are); with row_step set, row b draws with RNG counter row_step[b] + step on stream row_seq[b] instead of seq[b]
+  const int* active;
+  const uint32_t* row_step;
+  const uint32_t* row_seq;
   SampleSeq seq[64];
 };
 cudaError_t launch_sample(const SampleArgs& a, cudaStream_t s, uint64_t* counter);
@@ -243,6 +252,23 @@ struct SampleProc {
   int hist_stride;
 };
 cudaError_t launch_sample_proc(const SampleArgs& a, const SampleProc& q, cudaStream_t s, uint64_t* counter);
+// admission of a new sequence into row `row` of a running generation loop (one CTA, stream-ordered between two steps): draws
+// the row's first token from `logits` with the sampler arguments `a` (the loop's, with a.seq[row] = {suppress 1, step 0,
+// seq_id} and no loop state) and, with processors, the row's fresh history (already in q.hist) and eos_min; then writes the
+// row's decode state, RNG stream and counter base (1 - current step, so the n-th token after the first draws counter n),
+// appends the token to the history, activates the row and publishes (stamp << 32) | token to mailbox[row]
+struct SampleAdmit {
+  const float* logits;            // [V]
+  int row, slot, pos, share_slot, share_len, hist_len, eos_min;
+  uint32_t seq_id, stamp;
+  int *slots, *posv, *tok, *share_slots, *share_lens, *active;
+  uint32_t *row_step, *row_seq;
+  const unsigned long long* gen_step;
+  SampleProcTable* tab;           // with processors: eos_until[row] = eos_min
+  unsigned long long* mailbox;    // mapped pinned [max_batch]
+};
+cudaError_t launch_sample_admit(const SampleArgs& a, const SampleProc* q, const SampleAdmit& m, cudaStream_t s,
+                                uint64_t* counter);
 void set_sample_impl(int impl);   // 0 = register-resident kernel when V <= 32768 (default), 1 = generic kernel
 int get_sample_impl();
 

@@ -292,7 +292,8 @@ __global__ void __launch_bounds__(256) cast_bf16_f32_kernel(const bf16* __restri
 //      (HF modeling_llama.py:124-168; DynamicCache.update). grid (B, heads + 2*kv_heads); 64 threads.
 template <int HD>
 __global__ void __launch_bounds__(HD / 2) rope_kv_decode_kernel(const float* __restrict__ qkv, const int* __restrict__ slots,
-                                                                const int* __restrict__ posv, int heads, int kv_heads,
+                                                                const int* __restrict__ posv, const int* __restrict__ active,
+                                                                int heads, int kv_heads,
                                                                 const float* __restrict__ rope_cs, float* __restrict__ q_out,
                                                                 bf16* __restrict__ kv_base, int64_t kv_slot_stride,
                                                                 int64_t kv_v_offset, int max_len, bf16* __restrict__ q_bf16) {
@@ -313,6 +314,8 @@ __global__ void __launch_bounds__(HD / 2) rope_kv_decode_kernel(const float* __r
       d16[i] = __float2bfloat16_rn(y0);
       d16[i + HALF] = __float2bfloat16_rn(y1);
     }
+  } else if (active && !active[b]) {
+    // a retired row of a generation loop: its slot may already belong to another sequence
   } else if (hh < heads + kv_heads) {
     bf16* d = kv_base + (int64_t)slots[b] * kv_slot_stride + ((int64_t)(hh - heads) * max_len + pos) * HD;
     d[i] = __float2bfloat16_rn(a * cs.x - c * cs.y);
@@ -472,15 +475,15 @@ cudaError_t launch_cast_bf16_f32(const bf16* in, float* out, int64_t n, cudaStre
   if (counter) ++*counter;
   return cudaGetLastError();
 }
-cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, int heads, int kv_heads,
+cudaError_t launch_rope_kv_decode(const float* qkv, int B, const int* slots, const int* pos, const int* active, int heads, int kv_heads,
                                   const float* rope_cs, float* q_out, bf16* kv_base, int64_t kv_slot_stride,
                                   int64_t kv_v_offset, int max_len, int hd, cudaStream_t s, uint64_t* counter, bf16* q_bf16) {
   dim3 grid(B, heads + 2 * kv_heads);
   if (hd == 128)
-    rope_kv_decode_kernel<128><<<grid, 64, 0, s>>>(qkv, slots, pos, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
+    rope_kv_decode_kernel<128><<<grid, 64, 0, s>>>(qkv, slots, pos, active, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
                                                    kv_v_offset, max_len, q_bf16);
   else if (hd == 64)
-    rope_kv_decode_kernel<64><<<grid, 32, 0, s>>>(qkv, slots, pos, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
+    rope_kv_decode_kernel<64><<<grid, 32, 0, s>>>(qkv, slots, pos, active, heads, kv_heads, rope_cs, q_out, kv_base, kv_slot_stride,
                                                   kv_v_offset, max_len, q_bf16);
   else return cudaErrorInvalidValue;
   if (counter) ++*counter;

@@ -103,6 +103,13 @@ DTK_DEV float philox_uniform(uint64_t seed, uint32_t c0, uint32_t c1) {
   return (float)(x0 >> 8) * (1.0f / 16777216.0f);
 }
 
+// the uniform of row b: counter step + loop step on stream seq_id, from the loop's per-row arrays when it has them
+DTK_DEV float draw_uniform(const SampleArgs& p, const int b, const SampleSeq& sq) {
+  const uint32_t gstep = p.gen_step ? (uint32_t)*p.gen_step : 0u;
+  const uint32_t step = p.row_step ? p.row_step[b] : sq.step, sid = p.row_step ? p.row_seq[b] : sq.seq_id;
+  return philox_uniform(p.seed_dev ? *p.seed_dev : p.seed, step + gstep, sid);
+}
+
 // ---- HF logits processors (sampler instantiations with PROC = true only): the ban and repetition-penalty bitmasks of row
 // b, built from its token history h[0, L) and the call's tables in shared memory (2 x 4096 words, so V <= 131072).
 // HF generation/logits_process.py: RepetitionPenalty (every distinct id of input_ids), NoRepeatNGram
@@ -161,18 +168,18 @@ DTK_DEV void append_hist(const SampleProc& q, int b, int token) {
   q.hist_len[b] = min(L + 1, q.hist_stride);
 }
 
+// one row's token (every thread returns it) from logits lg with row b's state: scratch row, suppress flag, history and RNG
+// stream and counter (read at the draw: the loop's step counter advances only after every row of the step has arrived)
 template <bool PROC>
-DTK_DEV void sample_generic_body(const SampleArgs p, const SampleProc q) {
+DTK_DEV int sample_generic_body(const SampleArgs& p, const SampleProc& q, const int b, const float* lg) {
   __shared__ RedScratch red;
   __shared__ float sm_scan[32];
   __shared__ int sm_choice;
-  const int b = blockIdx.x, tid = threadIdx.x, V = p.V;
-  const float* lg = p.logits + (int64_t)b * V;
+  const int tid = threadIdx.x, V = p.V;
   float* w = p.scratch + (int64_t)b * V;
   const SampleSeq sq = p.seq[b];
   const bool sampling = p.do_sample && p.temperature > 0.f;
   const float T = sampling ? p.temperature : 1.f;
-  unsigned long long gstep = p.gen_step ? *p.gen_step : 0ull;
   uint32_t *ban = nullptr, *pen = nullptr;
   float penalty = 1.f, min_p = 0.f;
   if constexpr (PROC) {
@@ -265,8 +272,7 @@ DTK_DEV void sample_generic_body(const SampleArgs p, const SampleProc q) {
     for (int i = tid; i < V; i += ST) w[i] *= invz2;
     __syncthreads();
     // 6. inverse-CDF draw in index order
-    const uint32_t ctr = sq.step + (uint32_t)gstep;
-    const float u = philox_uniform(p.seed_dev ? *p.seed_dev : p.seed, ctr, sq.seq_id);
+    const float u = draw_uniform(p, b, sq);
     const int per = (V + ST - 1) / ST;
     const int i0 = tid * per, i1 = min(V, i0 + per);
     float loc = 0.f;
@@ -319,31 +325,49 @@ DTK_DEV void sample_generic_body(const SampleArgs p, const SampleProc q) {
     const float invz = 1.f / z;
     for (int i = tid; i < V; i += ST) w[i] *= invz;
   }
+  return token;
+}
 
-  if (tid == 0) {
-    if (p.out_ids) p.out_ids[b] = token;
-    if (p.gen_tok) {
+// thread 0 of row b's CTA, after the draw: the output id and the generation-loop state. A retired row (token -1, the ring's
+// sentinel) publishes only its stamped ring entry and its arrival, so the host and the step counter see every row every step
+template <bool PROC>
+DTK_DEV void finish_row(const SampleArgs& p, const SampleProc& q, const int b, const int token) {
+  if (p.out_ids) p.out_ids[b] = token;
+  if (p.gen_tok) {
+    const unsigned long long gstep = *p.gen_step;   // unchanged until this row has arrived below
+    if (token >= 0) {
       p.gen_tok[b] = token;
       p.gen_pos[b] = min(p.gen_pos[b] + 1, p.max_pos);
       if constexpr (PROC) append_hist(q, b, token);
-      // ONE 8-byte store to the mapped pinned ring carries the token and its step stamp, so no ordering between two
-      // host-visible stores (and no system-scope fence, a PCIe round trip) is needed; the host polls the entry itself
-      const unsigned long long entry = ((gstep + 1ull) << 32) | (unsigned long long)(unsigned)token;
-      asm volatile("st.relaxed.sys.global.u64 [%0], %1;\n" ::"l"(p.host_ring + (gstep % (unsigned long long)p.ring) * p.B + b), "l"(entry) : "memory");
-      unsigned prev = atomicAdd(p.done_counter, 1u);
-      if (prev == (unsigned)p.B - 1u) {   // last sequence of this step: advance the device-side step counter
-        *p.done_counter = 0u;
-        *p.gen_step = gstep + 1ull;
-      }
+    }
+    // ONE 8-byte store to the mapped pinned ring carries the token and its step stamp, so no ordering between two
+    // host-visible stores (and no system-scope fence, a PCIe round trip) is needed; the host polls the entry itself
+    const unsigned long long entry = ((gstep + 1ull) << 32) | (unsigned long long)(unsigned)token;
+    asm volatile("st.relaxed.sys.global.u64 [%0], %1;\n" ::"l"(p.host_ring + (gstep % (unsigned long long)p.ring) * p.B + b), "l"(entry) : "memory");
+    unsigned prev = atomicAdd(p.done_counter, 1u);
+    if (prev == (unsigned)p.B - 1u) {   // last sequence of this step: advance the device-side step counter
+      *p.done_counter = 0u;
+      *p.gen_step = gstep + 1ull;
     }
   }
 }
 
-__global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) {
-  sample_generic_body<false>(p, SampleProc{});
-}
-__global__ void __launch_bounds__(ST) sample_generic_proc_kernel(const SampleArgs p, const SampleProc q) {
-  sample_generic_body<true>(p, q);
+template <bool PROC>
+DTK_DEV int sample_body(const SampleArgs& p, const SampleProc& q, int b, const float* lg);
+
+// one CTA per row: the sampler of dtk_sample and of every generation-loop step
+template <bool REG, bool PROC>
+DTK_DEV void sample_row(const SampleArgs& p, const SampleProc& q) {
+  const int b = blockIdx.x;
+  if (p.active && !p.active[b]) {
+    if (threadIdx.x == 0) finish_row<PROC>(p, q, b, -1);
+    return;
+  }
+  const float* lg = p.logits + (int64_t)b * p.V;
+  int token;
+  if constexpr (REG) token = sample_body<PROC>(p, q, b, lg);
+  else token = sample_generic_body<PROC>(p, q, b, lg);
+  if (threadIdx.x == 0) finish_row<PROC>(p, q, b, token);
 }
 
 
@@ -379,18 +403,16 @@ DTK_DEV int allreduce_sum_int(int v, Red2& r, int& ph) {
 }
 
 template <bool PROC>
-DTK_DEV void sample_body(const SampleArgs p, const SampleProc q) {
+DTK_DEV int sample_body(const SampleArgs& p, const SampleProc& q, const int b, const float* lg) {
   __shared__ RedScratch red;
   __shared__ Red2 red2;
   __shared__ float sm_scan[32];
   __shared__ int sm_choice;
-  const int b = blockIdx.x, tid = threadIdx.x, V = p.V;
-  const float* lg = p.logits + (int64_t)b * V;
+  const int tid = threadIdx.x, V = p.V;
   float* w = p.scratch + (int64_t)b * V;
   const SampleSeq sq = p.seq[b];
   const bool sampling = p.do_sample && p.temperature > 0.f;
   const float T = sampling ? p.temperature : 1.f;
-  unsigned long long gstep = p.gen_step ? *p.gen_step : 0ull;
   int ph = 0;
   uint32_t *ban = nullptr, *pen = nullptr;
   float penalty = 1.f, min_p = 0.f;
@@ -493,8 +515,7 @@ DTK_DEV void sample_body(const SampleArgs p, const SampleProc q) {
       if (tid + j * ST < V) w[tid + j * ST] = v[j] * invz2;
     __syncthreads();
     // 6. inverse-CDF draw in index order (blocked ranges, read back from the scratch row)
-    const uint32_t ctr = sq.step + (uint32_t)gstep;
-    const float u = philox_uniform(p.seed_dev ? *p.seed_dev : p.seed, ctr, sq.seq_id);
+    const float u = draw_uniform(p, b, sq);
     const int per = (V + ST - 1) / ST;
     const int i0 = tid * per, i1 = min(V, i0 + per);
     float loc = 0.f;
@@ -549,28 +570,38 @@ DTK_DEV void sample_body(const SampleArgs p, const SampleProc q) {
     for (int j = 0; j < VPT; ++j)
       if (tid + j * ST < V) w[tid + j * ST] = v[j] * invz;
   }
-
-  if (tid == 0) {
-    if (p.out_ids) p.out_ids[b] = token;
-    if (p.gen_tok) {
-      p.gen_tok[b] = token;
-      p.gen_pos[b] = min(p.gen_pos[b] + 1, p.max_pos);
-      if constexpr (PROC) append_hist(q, b, token);
-      // ONE 8-byte store to the mapped pinned ring carries the token and its step stamp, so no ordering between two
-      // host-visible stores (and no system-scope fence, a PCIe round trip) is needed; the host polls the entry itself
-      const unsigned long long entry = ((gstep + 1ull) << 32) | (unsigned long long)(unsigned)token;
-      asm volatile("st.relaxed.sys.global.u64 [%0], %1;\n" ::"l"(p.host_ring + (gstep % (unsigned long long)p.ring) * p.B + b), "l"(entry) : "memory");
-      unsigned prev = atomicAdd(p.done_counter, 1u);
-      if (prev == (unsigned)p.B - 1u) {   // last sequence of this step: advance the device-side step counter
-        *p.done_counter = 0u;
-        *p.gen_step = gstep + 1ull;
-      }
-    }
-  }
+  return token;
 }
 
-__global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) { sample_body<false>(p, SampleProc{}); }
-__global__ void __launch_bounds__(ST) sample_proc_kernel(const SampleArgs p, const SampleProc q) { sample_body<true>(p, q); }
+__global__ void __launch_bounds__(ST) sample_generic_kernel(const SampleArgs p) { sample_row<false, false>(p, SampleProc{}); }
+__global__ void __launch_bounds__(ST) sample_generic_proc_kernel(const SampleArgs p, const SampleProc q) {
+  sample_row<false, true>(p, q);
+}
+__global__ void __launch_bounds__(ST) sample_kernel(const SampleArgs p) { sample_row<true, false>(p, SampleProc{}); }
+__global__ void __launch_bounds__(ST) sample_proc_kernel(const SampleArgs p, const SampleProc q) { sample_row<true, true>(p, q); }
+
+// admission of a sequence into row m.row of a running generation loop (launch_sample_admit)
+template <bool REG, bool PROC>
+__global__ void __launch_bounds__(ST) sample_admit_kernel(const SampleArgs p, const SampleProc q, const SampleAdmit m) {
+  const int r = m.row;
+  if constexpr (PROC) {   // the row's history (prompt) was copied in before this launch; its length and min-length here
+    if (threadIdx.x == 0) { q.hist_len[r] = m.hist_len; m.tab->eos_until[r] = m.eos_min; }
+    __syncthreads();
+  }
+  int token;   // counter p.seq[r].step (0) on stream p.seq[r].seq_id: p carries no loop state
+  if constexpr (REG) token = sample_body<PROC>(p, q, r, m.logits);
+  else token = sample_generic_body<PROC>(p, q, r, m.logits);
+  if (threadIdx.x == 0) {
+    const unsigned long long gstep = *m.gen_step;   // the loop step that decodes the first token draws counter 1
+    m.slots[r] = m.slot; m.posv[r] = m.pos; m.tok[r] = token;
+    m.share_slots[r] = m.share_slot; m.share_lens[r] = m.share_len;
+    m.row_step[r] = 1u - (uint32_t)gstep; m.row_seq[r] = m.seq_id;
+    if constexpr (PROC) append_hist(q, r, token);
+    m.active[r] = 1;
+    const unsigned long long entry = ((unsigned long long)m.stamp << 32) | (unsigned long long)(unsigned)token;
+    asm volatile("st.relaxed.sys.global.u64 [%0], %1;\n" ::"l"(m.mailbox + r), "l"(entry) : "memory");
+  }
+}
 
 }  // namespace
 
@@ -582,6 +613,22 @@ cudaError_t launch_sample(const SampleArgs& a, cudaStream_t s, uint64_t* counter
   if (a.B <= 0 || a.B > 64) return cudaErrorInvalidValue;
   if (g_sample_impl == 0 && a.V <= ST * VPT) sample_kernel<<<a.B, ST, 0, s>>>(a);
   else sample_generic_kernel<<<a.B, ST, 0, s>>>(a);
+  if (counter) ++*counter;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sample_admit(const SampleArgs& a, const SampleProc* q, const SampleAdmit& m, cudaStream_t s,
+                                uint64_t* counter) {
+  if (m.row < 0 || m.row >= 64 || (q && (a.V > kProcMaxVocab || !q->tab || !q->hist || !q->hist_len || !m.tab)))
+    return cudaErrorInvalidValue;
+  const bool reg = g_sample_impl == 0 && a.V <= ST * VPT;
+  if (q) {
+    if (reg) sample_admit_kernel<true, true><<<1, ST, 0, s>>>(a, *q, m);
+    else sample_admit_kernel<false, true><<<1, ST, 0, s>>>(a, *q, m);
+  } else {
+    if (reg) sample_admit_kernel<true, false><<<1, ST, 0, s>>>(a, SampleProc{}, m);
+    else sample_admit_kernel<false, false><<<1, ST, 0, s>>>(a, SampleProc{}, m);
+  }
   if (counter) ++*counter;
   return cudaGetLastError();
 }

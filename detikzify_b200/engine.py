@@ -216,7 +216,7 @@ class Engine:
         if self.device.type != "cuda":
             raise EngineError(f"unsupported device {self.device}")
         self.ccfg = to_c_config(cfg, max_seqs=max_seqs, max_batch=max_batch, max_len=max_len)
-        self.max_len = self.ccfg.max_len
+        self.max_len, self.max_batch = self.ccfg.max_len, self.ccfg.max_batch
         self.arena = arena.to(self.device, non_blocking=False).contiguous()
         self._h = C.c_void_p()
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
@@ -488,6 +488,24 @@ class Engine:
     def gen_wait(self, step: int) -> List[int]:
         self._check(self.lib.dtk_gen_wait(self._h, step, self._gen_out), "dtk_gen_wait")
         return list(self._gen_out)
+
+    def gen_admit(self, row: int, slot: int, position: int, logits: torch.Tensor, seq_id: int,
+                  history: Optional[Sequence[int]] = None, eos_min_len: int = 0):
+        """Put a new sequence into inactive row ``row`` of the running loop (``dtk_gen_admit``): ``slot`` holds its prompt up
+        to ``position``, ``logits`` fp32 [V] are the prompt's last-position logits; ``history`` (the prompt) and
+        ``eos_min_len`` matter while processors are set. The first token is drawn on the device; ``gen_first`` returns it."""
+        logits = logits.to(self.device, torch.float32).contiguous()
+        hist = list(history or [])
+        self._check(self.lib.dtk_gen_admit(self._h, row, slot, position, self._ptr(logits), C.c_uint32(seq_id), _i32(hist),
+                                           len(hist), int(eos_min_len), self._stream()), "dtk_gen_admit")
+
+    def gen_retire(self, row: int):
+        self._check(self.lib.dtk_gen_retire(self._h, row, self._stream()), "dtk_gen_retire")
+
+    def gen_first(self, row: int) -> int:
+        t = C.c_int32(0)
+        self._check(self.lib.dtk_gen_first(self._h, row, C.byref(t)), "dtk_gen_first")
+        return t.value
 
     def gen_end(self):
         self._check(self.lib.dtk_gen_end(self._h), "dtk_gen_end")

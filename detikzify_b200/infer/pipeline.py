@@ -494,5 +494,32 @@ class DetikzifyPipeline:
             docs.append(TikzDocument(code=code, timeout=timeout))
         return docs
 
+    def sample_many(self, images, samples_per_image: int = 1, batch_size: Optional[int] = None, preprocess: bool = True,
+                    **gen_kwargs) -> Generator[Tuple[int, TikzDocument], None, None]:
+        """``sample_batch`` for any number of figures and samples through one continuously refilled decode loop
+        (``model.generate_batch``'s kwargs and prompts, ``model.generate_many``): at most ``batch_size`` programs are decoded
+        at once and a finished one's row takes the next program at once. Each figure's samples share its image prefix.
+        Yields ``(index, document)`` in completion order; index ``i`` is sample ``i % samples_per_image`` of figure
+        ``i // samples_per_image``, as in ``sample_batch``'s image-major list."""
+        if not hasattr(self.model, "generate_many"):
+            raise TypeError("sample_many needs a detikzify_b200 model (generate_many)")
+        images = [self.load(im, preprocess=preprocess) for im in images]
+        kw = {**self.gen_kwargs, **gen_kwargs}
+        timeout = kw.pop("compile_timeout", 60)
+        prompts, pixels = [], []
+        for im in images:
+            enc = self.processor(images=im, text=None, return_tensors="pt")
+            pixels.append(enc["pixel_values"][0])
+            prompts += [enc.input_ids[0]] * samples_per_image
+        if not prompts:
+            return
+        figure = [i // samples_per_image for i in range(len(prompts))]
+        for i, ids in self.model.generate_many(
+                prompts, pixel_values=torch.stack(pixels), figure=figure, batch_size=batch_size,
+                bad_words_ids=[[self.model.config.image_token_id]],
+                begin_suppress_tokens=[self.model.config.text_config.eos_token_id], **kw):
+            code = self.processor.decode(token_ids=ids[len(prompts[i]):], skip_special_tokens=True)
+            yield i, TikzDocument(code=code, timeout=timeout)
+
     def __call__(self, *args, **kwargs) -> TikzDocument:
         return self.sample(*args, **kwargs)

@@ -25,9 +25,10 @@ expansion prefills only the tree-path suffix instead of re-encoding the image an
 from __future__ import annotations
 
 import threading
+from collections import deque
 from contextlib import nullcontext
 from types import SimpleNamespace
-from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, Iterator, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -145,6 +146,24 @@ class _KVSlot:
 
     def __init__(self, slot: int):
         self.slot, self.tokens, self.tick = slot, [], 0
+
+
+class _Requests:
+    """Per-sequence host state of a batched generation call (``generate_batch``, ``generate_many``): outputs, streamers,
+    stopping criteria and limits, and the rule by which a new token is accepted and a sequence stops."""
+
+    def __init__(self, prompts: List[List[int]], streamers, criteria: List[StoppingCriteriaList], limits: List[int], eos: int):
+        self.outs = [list(p) for p in prompts]
+        self.streamers, self.crits, self.limits, self.eos = streamers, criteria, limits, eos
+        self.done = [len(p) >= lim for p, lim in zip(prompts, limits)]   # prompt already at max_length: nothing appended
+
+    def accept(self, i: int, tok: int):
+        self.outs[i].append(tok)
+        if self.streamers[i] is not None:
+            self.streamers[i].put(torch.tensor([tok], dtype=torch.int64))
+        crit = self.crits[i]
+        cur = torch.tensor([self.outs[i]], dtype=torch.int64) if crit else None
+        self.done[i] = tok == self.eos or len(self.outs[i]) >= self.limits[i] or (bool(crit) and crit(cur, None))
 
 
 class DetikzifyForCausalLM:
@@ -542,6 +561,45 @@ class DetikzifyForCausalLM:
             return result
 
     # ---- batched generation (extension; the reference's generate() is batch-1) ---------------------
+    def _batch_sampling(self, temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
+                        kw: Dict[str, Any]) -> SimpleNamespace:
+        """The sampling and processor kwargs of a batched call, each falling back to ``generation_config``."""
+        gc = self.generation_config
+        g = SimpleNamespace(temperature=gc.temperature if temperature is None else temperature,
+                            top_p=gc.top_p if top_p is None else top_p, top_k=gc.top_k if top_k is None else top_k,
+                            do_sample=gc.do_sample if do_sample is None else do_sample,
+                            eos=self.config.eos_token_id if eos_token_id is None else eos_token_id)
+        g.procs = self._processors(bad_words_ids, begin_suppress_tokens, kw, g.eos,
+                                   bool(g.do_sample) and float(g.temperature) >= 1e-5)
+        return g
+
+    def _batch_params(self, g: SimpleNamespace, seed: Optional[int]):
+        self._call_counter += 1
+        return self.engine.sampling(
+            temperature=g.temperature, top_p=g.top_p, top_k=g.top_k or 0, do_sample=bool(g.do_sample),
+            bad_token=g.procs.bad_token, begin_suppress_token=g.procs.bs_token,
+            seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
+
+    def _batch_requests(self, prompts: List[List[int]], streamers, stopping_criteria, max_length, max_new_tokens,
+                        eos: int) -> _Requests:
+        """Per-sequence streamers (one entry or None each), stopping criteria (a callable or list per sequence, or one shared
+        entry) and ``max_length`` limits of N prompts."""
+        N, gc = len(prompts), self.generation_config
+        streamers = list(streamers) if streamers is not None else [None] * N
+        if len(streamers) != N:
+            raise ValueError("streamers must hold one entry (or None) per sequence")
+        crits: List[StoppingCriteriaList] = []
+        sc = list(stopping_criteria) if stopping_criteria is not None else []
+        per_seq = len(sc) == N and N > 1 or (len(sc) == N and all(isinstance(c, (list, tuple)) for c in sc))
+        for i in range(N):
+            c = sc[i] if per_seq else sc
+            crits.append(StoppingCriteriaList(c if isinstance(c, (list, tuple)) else [c]))
+        limits = []
+        for p in prompts:
+            ml = max_length if max_length is not None else (len(p) + max_new_tokens if max_new_tokens is not None else gc.max_length)
+            limits.append(min(int(ml), self.engine.max_len))
+        return _Requests(prompts, streamers, crits, limits, eos)
+
     @torch.no_grad()
     def generate_batch(self, input_ids: Sequence[torch.Tensor], pixel_values: Optional[torch.Tensor] = None, *,
                        bad_words_ids=None, begin_suppress_tokens=None, temperature: Optional[float] = None,
@@ -565,15 +623,10 @@ class DetikzifyForCausalLM:
         expansion) is prefilled ONCE and lent to every sequence (``dtk_seq_share``: reference counted, read in place);
         each sequence prefills only its own suffix. Returns a list of 1-D id tensors (prompt included).
         N is bounded by the engine's ``max_batch`` and free KV slots (``load(..., max_seqs=, max_batch=)``)."""
-        cfg, eng = self.config, self.engine
-        gc = self.generation_config
-        temperature = gc.temperature if temperature is None else temperature
-        top_p = gc.top_p if top_p is None else top_p
-        top_k = gc.top_k if top_k is None else top_k
-        do_sample = gc.do_sample if do_sample is None else do_sample
-        eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
-        procs = self._processors(bad_words_ids, begin_suppress_tokens, ignored, eos,
-                                 bool(do_sample) and float(temperature) >= 1e-5)
+        eng = self.engine
+        g = self._batch_sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
+                                 ignored)
+        procs = g.procs
         prompts: List[List[int]] = [(p[0] if p.dim() == 2 else p).tolist() for p in input_ids]
         N = len(prompts)
         if N == 0:
@@ -581,22 +634,10 @@ class DetikzifyForCausalLM:
         captions, pixel_values = self._batch_captions(adapter_input_ids, adapter_attention_mask, pixel_values, N)
         if any(len(p) == 0 for p in prompts):
             raise ValueError("empty prompt")
-        streamers = list(streamers) if streamers is not None else [None] * N
-        if len(streamers) != N:
-            raise ValueError("streamers must hold one entry (or None) per sequence")
-        crits: List[StoppingCriteriaList] = []
-        sc = list(stopping_criteria) if stopping_criteria is not None else []
-        per_seq = len(sc) == N and N > 1 or (len(sc) == N and all(isinstance(c, (list, tuple)) for c in sc))
-        for i in range(N):
-            c = sc[i] if per_seq else sc
-            crits.append(StoppingCriteriaList(c if isinstance(c, (list, tuple)) else [c]))
-        limits = []
-        for p in prompts:
-            ml = max_length if max_length is not None else (len(p) + max_new_tokens if max_new_tokens is not None else gc.max_length)
-            limits.append(min(int(ml), eng.max_len))
+        rq = self._batch_requests(prompts, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
         with self._lock, self._on_stream():
             imgs = self._batch_image_embeds(pixel_values, captions, N)
-            for i, st in enumerate(streamers):
+            for i, st in enumerate(rq.streamers):
                 if st is not None:
                     st.put(torch.tensor([prompts[i]], dtype=torch.int64))
             slots: List[int] = []
@@ -631,11 +672,7 @@ class DetikzifyForCausalLM:
                         eng.seq_share(base_slot, slots[i], lcp)
                     lg, _ = eng.prefill(slots[i], self._to_device_ids(ids_host[lcp:]), lcp, img, img_start)
                     last.append(lg)
-                self._call_counter += 1
-                params = eng.sampling(
-                    temperature=temperature, top_p=top_p, top_k=top_k or 0, do_sample=bool(do_sample),
-                    bad_token=procs.bad_token, begin_suppress_token=procs.bs_token,
-                    seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
+                params = self._batch_params(g, seed)
                 seq_ids = list(range(N))
                 eos_min = [procs.eos_min(len(p)) for p in prompts]
                 if procs.proc is not None:
@@ -643,41 +680,31 @@ class DetikzifyForCausalLM:
                     eng.set_processors(procs.proc, prompts, eos_min)
                 first, _ = eng.sample(torch.stack(last), params, suppress=[1] * N, steps=[0] * N, seq_ids=seq_ids)
                 toks = [int(t) for t in first.tolist()]
-                outs: List[List[int]] = [list(p) for p in prompts]
-                done = [len(p) >= lim for p, lim in zip(prompts, limits)]   # prompt already at max_length: nothing appended
-
-                def accept(i: int, tok: int):
-                    outs[i].append(tok)
-                    if streamers[i] is not None:
-                        streamers[i].put(torch.tensor([tok], dtype=torch.int64))
-                    cur = torch.tensor([outs[i]], dtype=torch.int64) if crits[i] else None
-                    done[i] = tok == eos or len(outs[i]) >= limits[i] or (bool(crits[i]) and crits[i](cur, None))
-
                 for i in range(N):
-                    if not done[i]:
-                        accept(i, toks[i])
-                max_steps = max(lim - len(p) for p, lim in zip(prompts, limits)) - 1
-                if not all(done) and max_steps > 0:
+                    if not rq.done[i]:
+                        rq.accept(i, toks[i])
+                max_steps = max(lim - len(p) for p, lim in zip(prompts, rq.limits)) - 1
+                if not all(rq.done) and max_steps > 0:
                     if procs.proc is not None:   # device histories continue from prompt + first token (at most max_len ids)
                         eng.set_processors(procs.proc, [(p + [t])[:eng.max_len] for p, t in zip(prompts, toks)], eos_min)
                     eng.gen_begin(slots, [len(p) for p in prompts], toks, params, seq_ids)
                     launched = waited = 0
                     try:
-                        while not all(done) and waited < max_steps:
+                        while not all(rq.done) and waited < max_steps:
                             while launched < waited + 2 and launched < max_steps:
                                 eng.gen_step()
                                 launched += 1
                             row = eng.gen_wait(waited)
                             waited += 1
                             for i in range(N):
-                                if not done[i]:          # finished sequences keep decoding on the device; the host ignores them
-                                    accept(i, int(row[i]))
+                                if not rq.done[i]:          # finished sequences keep decoding on the device; the host ignores them
+                                    rq.accept(i, int(row[i]))
                     finally:
                         eng.gen_end()
-                for st in streamers:
+                for st in rq.streamers:
                     if st is not None:
                         st.end()
-                result = [torch.tensor(o, dtype=torch.int64, device=self.device) for o in outs]
+                result = [torch.tensor(o, dtype=torch.int64, device=self.device) for o in rq.outs]
                 self._sync()
                 return result
             finally:
@@ -687,6 +714,240 @@ class DetikzifyForCausalLM:
                     eng.seq_free(s)
                 if base_slot is not None:
                     eng.seq_free(base_slot)
+
+    # ---- continuous batching (extension): a stream of requests through one running decode loop ---------
+    def generate_many(self, prompts: Sequence[torch.Tensor], pixel_values: Optional[torch.Tensor] = None, *,
+                      figure: Optional[Sequence[int]] = None, batch_size: Optional[int] = None, bad_words_ids=None,
+                      begin_suppress_tokens=None, temperature: Optional[float] = None, top_p: Optional[float] = None,
+                      top_k: Optional[int] = None, max_length: Optional[int] = None, max_new_tokens: Optional[int] = None,
+                      do_sample: Optional[bool] = None, seed: Optional[int] = None, eos_token_id: Optional[int] = None,
+                      streamers: Optional[Sequence[Any]] = None, stopping_criteria: Optional[Sequence[Any]] = None,
+                      adapter_input_ids=None, adapter_attention_mask=None, **ignored) -> Iterator[Tuple[int, torch.Tensor]]:
+        """Any number of independent sequences through ONE batched decode loop of at most ``batch_size`` rows (default and
+        upper bound: the engine's ``max_batch``; at least 2): when a sequence stops, its row is retired and the next queued
+        prompt is admitted into it while the loop runs on, so rows stay busy however much the programs' lengths vary.
+        Yields ``(index, ids)`` (ids: CPU int64 [T], prompt included) in completion order.
+
+        ``pixel_values`` [F,3,S,S] holds F figures and ``figure[i]`` names prompt i's (default: all share figure 0 when
+        F = 1, prompt i has figure i when F = N). The vision tower runs in batches of figures ahead of admission. Each
+        figure's longest common prompt prefix (``generate_batch``'s rule) is prefilled once into a base slot, lent to that
+        figure's sequences and freed after its last one stops; the loop uses shared-prefix (cascade) attention only when
+        every sequence borrows one prefix (one figure).
+
+        Per-sequence contract as ``generate_batch``: streamers, stopping criteria, EOS, ``max_length`` and RNG stream i of
+        ``seed`` for sequence i, so a sequence's tokens do not depend on when it was admitted; with one figure whose prompts
+        share the prefix the first ``batch_size`` share (e.g. samples of one prompt), those first ``batch_size`` sequences
+        equal ``generate_batch`` of their prompts. The model is busy until the generator is
+        exhausted or closed; slots and processors are released on every exit. TikZero captions are not supported."""
+        if adapter_input_ids is not None:
+            raise ValueError("generate_many() does not take TikZero captions (adapter_input_ids)")
+        eng = self.engine
+        B = eng.max_batch if batch_size is None else int(batch_size)
+        if not 2 <= B <= eng.max_batch:
+            raise ValueError(f"batch_size must lie in [2, max_batch = {eng.max_batch}], got {batch_size!r}")
+        g = self._batch_sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
+                                 ignored)
+        ids: List[List[int]] = [torch.as_tensor(p).reshape(-1).tolist() for p in prompts]
+        N = len(ids)
+        if any(len(p) == 0 for p in ids):
+            raise ValueError("empty prompt")
+        pix = None
+        if pixel_values is not None:
+            pix = pixel_values if pixel_values.dim() == 4 else pixel_values[None]
+        F = pix.shape[0] if pix is not None else 1
+        if figure is None:
+            if F not in (1, N):
+                raise ValueError("pixel_values must hold one figure (shared) or one per prompt, or pass `figure`")
+            figure = [0] * N if F == 1 else list(range(N))
+        figure = [int(f) for f in figure]
+        if len(figure) != N or any(not 0 <= f < F for f in figure):
+            raise ValueError(f"figure must hold one index in [0, {F}) per prompt")
+        rq = self._batch_requests(ids, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
+        return self._many(ids, pix, figure, B, g, seed, rq)
+
+    def _many(self, prompts: List[List[int]], pix: Optional[torch.Tensor], figure: List[int], B: int, g: SimpleNamespace,
+              seed: Optional[int], rq: _Requests) -> Iterator[Tuple[int, torch.Tensor]]:
+        eng, procs, N = self.engine, g.procs, len(prompts)
+        spans = [self._image_span(p) if pix is not None else (0, 0) for p in prompts]
+        members: Dict[int, List[int]] = {}
+        for i, f in enumerate(figure):
+            members.setdefault(f, []).append(i)
+        left = {f: len(m) for f, m in members.items()}    # sequences of the figure that have not stopped
+        bases: Dict[int, Tuple[Optional[int], int]] = {}   # figure -> (base slot, shared length) once its first one is admitted
+        embeds: Dict[int, torch.Tensor] = {}
+        queue = deque(range(N))
+        slot_of: Dict[int, int] = {}
+        rows: List[Optional[int]] = []       # occupant of each loop row (None = retired)
+        s0: List[int] = []                   # step from which the ring's entry of a row belongs to its occupant
+        finished: List[Tuple[int, torch.Tensor]] = []
+        state = dict(begun=False, procs=False, cascade=None)
+
+        def figure_embeds(f: int) -> torch.Tensor:
+            if f not in embeds:                                # the tower runs for the next figures in queue order
+                todo = [f] + [h for h in dict.fromkeys(figure[i] for i in queue) if h != f and h not in embeds]
+                todo = todo[:8]
+                out = eng.image_embeds(pix[todo].to(self.device, torch.float32))
+                for k, h in enumerate(todo):
+                    embeds[h] = out[k]
+            return embeds[f]
+
+        def figure_prefix(f: int) -> Tuple[Optional[int], int]:
+            if f not in bases:
+                ps = [prompts[i] for i in members[f]]
+                lcp = self._shared_prefix(ps, min(len(p) for p in ps) - 1, spans[members[f][0]]) if len(ps) > 1 else 0
+                base = None
+                if lcp:
+                    try:
+                        base = eng.seq_alloc()
+                    except Exception:       # no spare slot: the figure's sequences prefill their whole prompts
+                        lcp = 0
+                if lcp:
+                    st0, n0 = spans[members[f][0]]
+                    img = figure_embeds(f) if (pix is not None and n0 and st0 < lcp) else None
+                    eng.prefill(base, self._to_device_ids(prompts[members[f][0]][:lcp]), 0, img, st0)
+                bases[f] = (base, lcp)
+            return bases[f]
+
+        def prefill(i: int, slot: int) -> torch.Tensor:
+            """prompt i into its slot after the figure's shared prefix; the last position's logits"""
+            f = figure[i]
+            base, lcp = figure_prefix(f)
+            img_start, n_patch = spans[i]
+            img = figure_embeds(f) if (pix is not None and n_patch and img_start >= lcp) else None
+            if lcp:
+                eng.seq_share(base, slot, lcp)
+            lg, _ = eng.prefill(slot, self._to_device_ids(prompts[i][lcp:]), lcp, img, img_start)
+            return lg
+
+        def stop(i: int):
+            """sequence i is complete: release its slot (and its figure's base after the last one) and queue its result"""
+            if i in slot_of:
+                eng.seq_free(slot_of.pop(i))
+            f = figure[i]
+            left[f] -= 1
+            if left[f] == 0:
+                base, _ = bases.pop(f, (None, 0))
+                if base is not None:
+                    eng.seq_free(base)
+                embeds.pop(f, None)
+            if rq.streamers[i] is not None:
+                rq.streamers[i].end()
+            finished.append((i, torch.tensor(rq.outs[i], dtype=torch.int64)))
+
+        def put_prompt(i: int):
+            if rq.streamers[i] is not None:
+                rq.streamers[i].put(torch.tensor([prompts[i]], dtype=torch.int64))
+
+        self._lock.acquire()
+        ctx = self._on_stream()
+        ctx.__enter__()
+        try:
+            # ---- first wave: exactly generate_batch's calls for the first batch_size prompts
+            wave = [queue.popleft() for _ in range(min(B, N))]
+            if pix is not None:
+                for f in dict.fromkeys(figure[i] for i in wave):
+                    figure_embeds(f)
+            for i in wave:
+                put_prompt(i)
+            for i in wave:
+                slot_of[i] = eng.seq_alloc()
+            last = [prefill(i, slot_of[i]) for i in wave]
+            params = self._batch_params(g, seed)
+            eos_min = [procs.eos_min(len(prompts[i])) for i in wave]
+            if procs.proc is not None:
+                state["procs"] = True
+                eng.set_processors(procs.proc, [prompts[i] for i in wave], eos_min)
+            first, _ = eng.sample(torch.stack(last), params, suppress=[1] * len(wave), steps=[0] * len(wave), seq_ids=wave)
+            toks = [int(t) for t in first.tolist()]
+            for i, t in zip(wave, toks):
+                if not rq.done[i]:
+                    rq.accept(i, t)
+            # steps the admitted sequences can use at most (a sequence admitted at step s0 takes its last token from step
+            # s0 + limit - len(prompt) - 2); as in generate_batch, no step is launched beyond the longest of them
+            cap = max(rq.limits[i] - len(prompts[i]) for i in wave) - 1
+            if (not all(rq.done[i] for i in wave) and cap > 0) or queue:
+                if procs.proc is not None:
+                    eng.set_processors(procs.proc, [(prompts[i] + [t])[:eng.max_len] for i, t in zip(wave, toks)], eos_min)
+                if len(members) > 1 and state["cascade"] is None:   # one shared prefix per figure: per-row reads only
+                    state["cascade"] = eng.get_option("cascade_attn")
+                    eng.set_option("cascade_attn", 0)
+                eng.gen_begin([slot_of[i] for i in wave], [len(prompts[i]) for i in wave], toks, params, wave)
+                state["begun"] = True
+                rows, s0 = list(wave), [0] * len(wave)
+            launched = waited = 0
+            pending: List[int] = []              # rows admitted since the last step launch: first token not read yet
+            while True:
+                for r, i in enumerate(rows):
+                    if i is not None and rq.done[i]:
+                        eng.gen_retire(r)
+                        rows[r] = None
+                        stop(i)
+                if not state["begun"]:
+                    for i in wave:
+                        stop(i)
+                # admissions into free rows; a prompt already at its limit completes without one
+                for r in range(len(rows)):
+                    while rows[r] is None and queue:
+                        i = queue[0]
+                        if rq.done[i]:
+                            queue.popleft()
+                            put_prompt(i)
+                            stop(i)
+                            continue
+                        try:
+                            slot = eng.seq_alloc()
+                        except Exception:
+                            if any(o is not None for o in rows):
+                                break               # wait for a slot to be released
+                            raise
+                        queue.popleft()
+                        slot_of[i] = slot
+                        put_prompt(i)
+                        lg = prefill(i, slot)
+                        eng.gen_admit(r, slot, len(prompts[i]), lg, i,
+                                      prompts[i] if procs.proc is not None else None, procs.eos_min(len(prompts[i])))
+                        rows[r], s0[r] = i, launched
+                        cap = max(cap, launched + rq.limits[i] - len(prompts[i]) - 1)
+                        pending.append(r)
+                if finished:
+                    out, finished[:] = list(finished), []
+                    ctx.__exit__(None, None, None)
+                    try:
+                        yield from out
+                    finally:
+                        ctx = self._on_stream()
+                        ctx.__enter__()
+                if all(i is None for i in rows):
+                    break
+                while launched < waited + 2 and launched < cap:
+                    eng.gen_step()
+                    launched += 1
+                for r in pending:                    # the admission kernels ran before the steps just launched
+                    rq.accept(rows[r], eng.gen_first(r))
+                pending = []
+                if not any(i is not None and not rq.done[i] for i in rows):
+                    continue
+                row = eng.gen_wait(waited)
+                for r, i in enumerate(rows):
+                    if i is not None and waited >= s0[r] and not rq.done[i]:
+                        rq.accept(i, int(row[r]))
+                waited += 1
+        finally:
+            try:
+                if state["begun"]:
+                    eng.gen_end()
+                if state["cascade"] is not None:
+                    eng.set_option("cascade_attn", state["cascade"])
+                if state["procs"]:
+                    eng.set_processors(None)
+                for slot in slot_of.values():
+                    eng.seq_free(slot)
+                for base, _ in bases.values():
+                    if base is not None:
+                        eng.seq_free(base)
+            finally:
+                ctx.__exit__(None, None, None)
+                self._lock.release()
 
     # ---- logits, loss and sequence scoring ---------------------------------------------------------
     def __call__(self, *args, **kwargs):

@@ -254,6 +254,28 @@ DTK_API int dtk_gen_step(dtk_engine* eng, void* stream);
 DTK_API int dtk_gen_wait(dtk_engine* eng, int64_t step, int32_t* tokens_out_host /* [B] */);
 DTK_API int dtk_gen_end(dtk_engine* eng);
 
+/* ---- continuous batching: change a row's occupant while the loop runs (batched loops, B >= 2 or the per-op B = 1 loop).
+ *      dtk_gen_retire: row `row` stops; every step launched after the call leaves its slot untouched (no KV write, no key
+ *      read) and publishes the sentinel token -1 for it (dtk_gen_wait still returns every row of every step).
+ *      dtk_gen_admit: row `row` (inactive) takes a new sequence whose prompt is prefilled into `slot` up to `position`
+ *      (shared-prefix state as the slot has it); `logits` device fp32 [V] are the prompt's last-position logits. The call
+ *      enqueues one kernel that draws the first token with the loop's sampling parameters (begin-suppress on, RNG counter 0
+ *      on stream seq_id), writes the row's state and activates it; the n-th token after the first draws counter n, so the
+ *      sequence draws exactly what a loop of its own would. With processors set the row's history becomes hist_ids[0,
+ *      hist_len) (host; it must end with the prompt) plus the first token, and EOS is banned while it is shorter than
+ *      eos_min_len; without them both are ignored. DTK_ERR_UNSUPPORTED on the batch-1 persistent loop; DTK_ERR_INVALID for
+ *      an active row, an unallocated slot, a position inside a shared prefix, another stream than the loop's, and on a
+ *      loop begun with shared-prefix (cascade) attention a slot that does not borrow exactly that loop's prefix.
+ *      dtk_gen_first: waits for the admitted row's first token (as dtk_gen_wait waits for a step).
+ *      Ordering: every device effect is ordered on the loop's stream behind the steps already launched, so the host may
+ *      dtk_seq_free a retired row's slot at once and reuse it (a prefill into it runs after those steps). A step launched
+ *      before the retirement decodes the row once more, at positions beyond the end of its sequence. A sequence admitted
+ *      when s steps have been launched appears in the ring from step s on. -------------------------------------------- */
+DTK_API int dtk_gen_admit(dtk_engine* eng, int row, int slot, int position, const float* logits, uint32_t seq_id,
+                          const int32_t* hist_ids, int hist_len, int eos_min_len, void* stream);
+DTK_API int dtk_gen_retire(dtk_engine* eng, int row, void* stream);
+DTK_API int dtk_gen_first(dtk_engine* eng, int row, int32_t* token_out_host);
+
 /* ---- engine options. "decode_impl": 1 = persistent weight-streaming decode kernel (default for
  *      B = 1), 0 = per-op kernels replayed from a CUDA graph (always used for B > 1). Others (all with
  *      working defaults): "gemm_impl" (see dtk_dbg_gemm_impl), "attn_impl" (ViT attention: 1 = wgmma, 0 =
