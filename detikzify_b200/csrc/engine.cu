@@ -1645,24 +1645,30 @@ int dtk_score(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_po
   return DTK_OK;
 }
 
+// Validates row i of a decode step or loop (slot in range, position below max_len and past every shared prefix: the
+// slot's own borrowed one and any it lends) and fills its StateArgs entry, including the prefix it reads through.
+static int fill_row(dtk_engine* eng, StateArgs& st, int i, int slot, int position) {
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(slot >= 0 && slot < c.max_seqs, "slot");
+  DTK_REQUIRE(position >= 0 && position < c.max_len, "position exceeds max_len");
+  DTK_REQUIRE(position >= eng->share_len[slot] && position >= eng->shared_upto[slot],
+              "position lies inside a shared prefix (one the slot borrows, or one it lends to other sequences)");
+  st.slots[i] = slot;
+  st.pos[i] = position;
+  st.share_slot[i] = eng->share_base[slot] >= 0 ? eng->share_base[slot] : slot;
+  st.share_len[i] = eng->share_len[slot];
+  return DTK_OK;
+}
+
 int dtk_decode(dtk_engine* eng, const int* slots, const int* positions, const int64_t* ids, int B, float* logits,
                void* stream) {
   if (!eng) return DTK_ERR_INVALID;
-  const dtk_config& c = eng->cfg;
   DTK_REQUIRE(slots && positions && ids && logits, "null pointer");
-  DTK_REQUIRE(B > 0 && B <= c.max_batch, "B exceeds max_batch");
+  DTK_REQUIRE(B > 0 && B <= eng->cfg.max_batch, "B exceeds max_batch");
   StateArgs st{};
   st.n = B;
-  for (int i = 0; i < B; ++i) {
-    DTK_REQUIRE(slots[i] >= 0 && slots[i] < c.max_seqs, "slot");
-    DTK_REQUIRE(positions[i] >= 0 && positions[i] < c.max_len, "position exceeds max_len");
-    DTK_REQUIRE(positions[i] >= eng->share_len[slots[i]], "position lies inside the sequence's shared (read-only) prefix");
-    DTK_REQUIRE(positions[i] >= eng->shared_upto[slots[i]], "position lies inside a prefix other sequences share from this slot");
-    st.slots[i] = slots[i];
-    st.pos[i] = positions[i];
-    st.share_slot[i] = eng->share_base[slots[i]] >= 0 ? eng->share_base[slots[i]] : slots[i];
-    st.share_len[i] = eng->share_len[slots[i]];
-  }
+  for (int i = 0; i < B; ++i)
+    if (int r = fill_row(eng, st, i, slots[i], positions[i])) return r;
   DTK_CK(cudaSetDevice(eng->device));
   cudaStream_t s = (cudaStream_t)stream;
   set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_active,
@@ -1742,12 +1748,8 @@ int dtk_gen_begin(dtk_engine* eng, const int* slots, const int* positions, const
   StateArgs st{};
   st.n = B; st.have_tok = 1;
   for (int i = 0; i < B; ++i) {
-    DTK_REQUIRE(slots[i] >= 0 && slots[i] < c.max_seqs, "slot");
-    DTK_REQUIRE(positions[i] >= 0 && positions[i] < c.max_len, "position exceeds max_len");
-    DTK_REQUIRE(positions[i] >= eng->share_len[slots[i]] && positions[i] >= eng->shared_upto[slots[i]], "position lies inside a shared prefix");
-    st.slots[i] = slots[i]; st.pos[i] = positions[i]; st.tok[i] = first_ids_host[i]; st.seq[i] = seq_ids ? seq_ids[i] : (uint32_t)i;
-    st.share_slot[i] = eng->share_base[slots[i]] >= 0 ? eng->share_base[slots[i]] : slots[i];
-    st.share_len[i] = eng->share_len[slots[i]];
+    if (int r = fill_row(eng, st, i, slots[i], positions[i])) return r;
+    st.tok[i] = first_ids_host[i]; st.seq[i] = seq_ids ? seq_ids[i] : (uint32_t)i;
   }
   set_cascade(eng, st);
   set_state_kernel<<<1, 64, 0, s>>>(st, eng->d_slots, eng->d_pos, eng->d_tok, eng->d_share_slot, eng->d_share_len, eng->d_active,
@@ -1834,39 +1836,48 @@ int dtk_gen_step(dtk_engine* eng, void* stream) {
   return DTK_OK;
 }
 
+// Spins until the host-ring entry *e carries the stamp `want` in its upper half (one 8-byte device store) and returns its
+// lower half, the token. Every 1024 spins it checks the loop's stream for an error, for running idle without the store,
+// and for 60 s gone since t0. With `ring`, a larger stamp means the device overwrote the entry a whole ring ahead.
+static int wait_stamped(dtk_engine* eng, volatile const unsigned long long* e, unsigned long long want, bool ring,
+                        const char* what, std::chrono::steady_clock::time_point t0, int32_t* token_out) {
+  uint64_t spins = 0;
+  unsigned long long v;
+  while (((v = *e) >> 32) != want) {
+    if (ring && (v >> 32) > want) {
+      eng->err = "token ring overrun: dtk_gen_wait lagged more than the ring depth behind dtk_gen_step";
+      return DTK_ERR_INVALID;
+    }
+    if ((++spins & 0x3ff) == 0) {
+      cudaError_t q = cudaStreamQuery(eng->gen_stream);
+      if (q != cudaSuccess && q != cudaErrorNotReady) {
+        eng->err = std::string("stream error while waiting for ") + what + ": " + cudaGetErrorString(q);
+        return DTK_ERR_CUDA;
+      }
+      if (q == cudaSuccess && (*e >> 32) != want) {
+        eng->err = std::string("stream idle but ") + what + " was never published";
+        return DTK_ERR_INVALID;
+      }
+      if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(60)) {
+        eng->err = std::string("timeout waiting for ") + what;
+        return DTK_ERR_CUDA;
+      }
+    }
+  }
+  *token_out = (int32_t)(uint32_t)(v & 0xffffffffull);
+  return DTK_OK;
+}
+
 int dtk_gen_wait(dtk_engine* eng, int64_t step, int32_t* tokens_out_host) {
   if (!eng) return DTK_ERR_INVALID;
   DTK_REQUIRE(eng->gen_B > 0 && step >= 0 && tokens_out_host, "gen state/step/out");
-  // every sequence's entry of this step carries the stamp step + 1 in its upper half (one 8-byte device store)
+  // every sequence's entry of this step carries the stamp step + 1
   volatile const unsigned long long* row = eng->host_ring + (size_t)(step % eng->ring) * eng->gen_B;
-  const unsigned long long want = (unsigned long long)(step + 1);
   auto t0 = std::chrono::steady_clock::now();
-  uint64_t spins = 0;
-  for (int i = 0; i < eng->gen_B; ++i) {
-    unsigned long long e;
-    while (((e = row[i]) >> 32) != want) {
-      if ((e >> 32) > want) {   // the device is a whole ring ahead: the token was overwritten
-        eng->err = "token ring overrun: dtk_gen_wait lagged more than the ring depth behind dtk_gen_step";
-        return DTK_ERR_INVALID;
-      }
-      if ((++spins & 0x3ff) == 0) {
-        cudaError_t q = cudaStreamQuery(eng->gen_stream);
-        if (q != cudaSuccess && q != cudaErrorNotReady) {
-          eng->err = std::string("stream error while waiting for token: ") + cudaGetErrorString(q);
-          return DTK_ERR_CUDA;
-        }
-        if (q == cudaSuccess && (row[i] >> 32) != want) {
-          eng->err = "stream idle but requested step was never launched";
-          return DTK_ERR_INVALID;
-        }
-        if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(60)) {
-          eng->err = "timeout waiting for generated token";
-          return DTK_ERR_CUDA;
-        }
-      }
-    }
-    tokens_out_host[i] = (int32_t)(uint32_t)(e & 0xffffffffull);
-  }
+  for (int i = 0; i < eng->gen_B; ++i)
+    if (int r = wait_stamped(eng, row + i, (unsigned long long)(step + 1), true, "the generated token", t0,
+                             tokens_out_host + i))
+      return r;
   return DTK_OK;
 }
 
@@ -1883,10 +1894,10 @@ int dtk_gen_admit(dtk_engine* eng, int row, int slot, int position, const float*
   DTK_REQUIRE(row >= 0 && row < eng->gen_B, "row outside the loop's rows");
   DTK_REQUIRE(!eng->row_active[row], "row is active (dtk_gen_retire it first)");
   DTK_REQUIRE(slot >= 0 && slot < c.max_seqs && eng->slot_used[slot], "slot is not allocated");
-  DTK_REQUIRE(position >= 0 && position < c.max_len, "position exceeds max_len");
-  DTK_REQUIRE(position >= eng->share_len[slot] && position >= eng->shared_upto[slot], "position lies inside a shared prefix");
+  StateArgs st{};
+  if (int r = fill_row(eng, st, 0, slot, position)) return r;
   DTK_REQUIRE(logits, "null logits");
-  const int share_slot = eng->share_base[slot] >= 0 ? eng->share_base[slot] : slot, share_len = eng->share_len[slot];
+  const int share_slot = st.share_slot[0], share_len = st.share_len[0];
   // the shared-prefix attention of this loop's graph reads one baked prefix for every row
   DTK_REQUIRE(eng->cas_len == 0 || (share_slot == eng->cas_slot && share_len == eng->cas_len),
               "the loop runs shared-prefix (cascade) attention over another prefix than the slot borrows");
@@ -1946,30 +1957,8 @@ int dtk_gen_first(dtk_engine* eng, int row, int32_t* token_out_host) {
   if (!eng) return DTK_ERR_INVALID;
   DTK_REQUIRE(eng->gen_B > 0 && token_out_host, "gen state/out");
   DTK_REQUIRE(row >= 0 && row < eng->gen_B && eng->admit_stamp[row] > 0, "row was not admitted in this loop");
-  volatile const unsigned long long* box = eng->host_ring + (size_t)eng->ring * 64 + row;
-  const unsigned long long want = eng->admit_stamp[row];
-  auto t0 = std::chrono::steady_clock::now();
-  uint64_t spins = 0;
-  unsigned long long e;
-  while (((e = *box) >> 32) != want) {
-    if ((++spins & 0x3ff) == 0) {
-      cudaError_t q = cudaStreamQuery(eng->gen_stream);
-      if (q != cudaSuccess && q != cudaErrorNotReady) {
-        eng->err = std::string("stream error while waiting for an admitted row's first token: ") + cudaGetErrorString(q);
-        return DTK_ERR_CUDA;
-      }
-      if (q == cudaSuccess && (*box >> 32) != want) {
-        eng->err = "stream idle but the admission never published its first token";
-        return DTK_ERR_INVALID;
-      }
-      if (std::chrono::steady_clock::now() - t0 > std::chrono::seconds(60)) {
-        eng->err = "timeout waiting for an admitted row's first token";
-        return DTK_ERR_CUDA;
-      }
-    }
-  }
-  *token_out_host = (int32_t)(uint32_t)(e & 0xffffffffull);
-  return DTK_OK;
+  return wait_stamped(eng, eng->host_ring + (size_t)eng->ring * 64 + row, eng->admit_stamp[row], false,
+                      "an admitted row's first token", std::chrono::steady_clock::now(), token_out_host);
 }
 
 int dtk_gen_end(dtk_engine* eng) {

@@ -149,21 +149,156 @@ class _KVSlot:
 
 
 class _Requests:
-    """Per-sequence host state of a batched generation call (``generate_batch``, ``generate_many``): outputs, streamers,
-    stopping criteria and limits, and the rule by which a new token is accepted and a sequence stops."""
+    """Per-sequence host state of a generation call: each request's ids (an int64 [1, limit] CPU buffer, allocated when the
+    request starts), streamers, stopping criteria and limits, and the rule by which a new token is accepted and a sequence
+    stops. Criteria see a [1, T] view of the buffer; streamers get the prompt as [1, T0] and every new token as [1]."""
 
     def __init__(self, prompts: List[List[int]], streamers, criteria: List[StoppingCriteriaList], limits: List[int], eos: int):
-        self.outs = [list(p) for p in prompts]
-        self.streamers, self.crits, self.limits, self.eos = streamers, criteria, limits, eos
+        self.prompts, self.streamers, self.crits, self.limits, self.eos = prompts, streamers, criteria, limits, eos
+        self.bufs: List[Optional[torch.Tensor]] = [None] * len(prompts)
+        self.lens = [len(p) for p in prompts]
         self.done = [len(p) >= lim for p, lim in zip(prompts, limits)]   # prompt already at max_length: nothing appended
 
-    def accept(self, i: int, tok: int):
-        self.outs[i].append(tok)
+    def start(self, i: int):
+        p = self.prompts[i]
+        self.bufs[i] = torch.empty(1, max(self.limits[i], len(p)), dtype=torch.int64)
+        self.bufs[i][0, : len(p)] = torch.tensor(p, dtype=torch.int64)
         if self.streamers[i] is not None:
-            self.streamers[i].put(torch.tensor([tok], dtype=torch.int64))
+            self.streamers[i].put(self.ids(i))
+
+    def ids(self, i: int) -> torch.Tensor:
+        return self.bufs[i][:, : self.lens[i]]
+
+    def accept(self, i: int, tok: int):
+        n = self.lens[i]
+        self.bufs[i][0, n] = tok
+        self.lens[i] = n + 1
+        if self.streamers[i] is not None:
+            self.streamers[i].put(self.bufs[i][0, n: n + 1])
         crit = self.crits[i]
-        cur = torch.tensor([self.outs[i]], dtype=torch.int64) if crit else None
-        self.done[i] = tok == self.eos or len(self.outs[i]) >= self.limits[i] or (bool(crit) and crit(cur, None))
+        self.done[i] = tok == self.eos or n + 1 >= self.limits[i] or (bool(crit) and crit(self.ids(i), None))
+
+    def end(self, i: int):
+        if self.streamers[i] is not None:
+            self.streamers[i].end()
+
+
+class _DecodeLoop:
+    """The host side of one fused generation loop over the requests ``rq``, for ``generate`` (one row), ``generate_batch``
+    (N rows) and ``generate_many`` (a queue). ``run(wave, logits)`` draws the first tokens of the requests ``wave``, whose
+    prompts ``slots`` hold and end in ``logits``, begins the loop and keeps two steps in flight until every row has stopped.
+    With a ``queue`` a stopped row is retired (slot freed, then ``release(i)``), the next request admitted into it
+    (``prefill(i, slot)`` -> its logits) and ``run`` yields the requests completed since its last yield; without one,
+    finished rows decode on unread. ``per_row_attn`` turns the shared-prefix cascade off while the loop runs. Every exit
+    ends the loop and restores the cascade option and processors. ``launched``: steps launched so far."""
+
+    def __init__(self, model: "DetikzifyForCausalLM", rq: _Requests, g: SimpleNamespace, seed: Optional[int],
+                 slots: Dict[int, int], queue: Optional[deque] = None, prefill=None, release=None,
+                 per_row_attn: bool = False):
+        self.model, self.rq, self.g, self.seed, self.slots = model, rq, g, seed, slots
+        self.queue, self.prefill, self.release, self.per_row_attn = queue, prefill, release, per_row_attn
+        self.launched = 0
+
+    def run(self, wave: List[int], logits: List[torch.Tensor]) -> Iterator[List[int]]:
+        eng, rq, procs, queue = self.model.engine, self.rq, self.g.procs, self.queue
+        params = self.model._sampling_params(self.g, self.seed)
+        rows: List[Optional[int]] = list(wave)   # occupant of each loop row (None = retired)
+        s0 = [0] * len(wave)                      # step from which the ring's entry of a row belongs to its occupant
+        pending: List[int] = []                   # rows admitted since the last step launch: first token not read yet
+        finished: List[int] = []
+        begun, cascade = False, None
+        try:
+            eos_min = [procs.eos_min(len(rq.prompts[i])) for i in wave]
+            if procs.proc is not None:
+                eng.set_processors(procs.proc, [rq.prompts[i] for i in wave], eos_min)
+            first, _ = eng.sample(torch.stack(logits), params, suppress=[1] * len(wave), steps=[0] * len(wave),
+                                  seq_ids=wave)
+            toks = [int(t) for t in first.tolist()]
+            for i, t in zip(wave, toks):
+                if not rq.done[i]:
+                    rq.accept(i, t)
+            # steps the admitted sequences can use at most (a sequence admitted at step s0 takes its last token from step
+            # s0 + limit - len(prompt) - 2); no step is launched beyond the longest of them
+            cap = max(rq.limits[i] - len(rq.prompts[i]) for i in wave) - 1
+            if (not all(rq.done[i] for i in wave) and cap > 0) or queue:
+                if procs.proc is not None:   # device histories continue from prompt + first token (at most max_len ids)
+                    eng.set_processors(procs.proc, [(rq.prompts[i] + [t])[:eng.max_len] for i, t in zip(wave, toks)],
+                                       eos_min)
+                if self.per_row_attn:
+                    cascade = eng.get_option("cascade_attn")
+                    eng.set_option("cascade_attn", 0)
+                eng.gen_begin([self.slots[i] for i in wave], [len(rq.prompts[i]) for i in wave], toks, params, wave)
+                begun = True
+            waited = 0
+            while True:
+                if queue is not None:
+                    for r, i in enumerate(rows):
+                        if i is not None and rq.done[i]:
+                            if begun:
+                                eng.gen_retire(r)
+                            rows[r] = None
+                            self._stop(i, finished)
+                    # admissions into free rows; a prompt already at its limit completes without one
+                    for r in range(len(rows)):
+                        while rows[r] is None and queue:
+                            i = queue[0]
+                            if rq.done[i]:
+                                queue.popleft()
+                                rq.start(i)
+                                self._stop(i, finished)
+                                continue
+                            try:
+                                slot = eng.seq_alloc()
+                            except Exception:
+                                if any(o is not None for o in rows):
+                                    break               # wait for a slot to be released
+                                raise
+                            queue.popleft()
+                            self.slots[i] = slot
+                            rq.start(i)
+                            lg = self.prefill(i, slot)
+                            p = rq.prompts[i]
+                            eng.gen_admit(r, slot, len(p), lg, i, p if procs.proc is not None else None,
+                                          procs.eos_min(len(p)))
+                            rows[r], s0[r] = i, self.launched
+                            cap = max(cap, self.launched + rq.limits[i] - len(p) - 1)
+                            pending.append(r)
+                    if finished:
+                        out, finished = finished, []
+                        yield out
+                if all(i is None or rq.done[i] for i in rows):
+                    break
+                while self.launched < waited + 2 and self.launched < cap:
+                    eng.gen_step()
+                    self.launched += 1
+                for r in pending:                    # the admission kernels ran before the steps just launched
+                    rq.accept(rows[r], eng.gen_first(r))
+                pending = []
+                if not any(i is not None and not rq.done[i] for i in rows):
+                    continue
+                row = eng.gen_wait(waited)
+                for r, i in enumerate(rows):
+                    if i is not None and waited >= s0[r] and not rq.done[i]:
+                        rq.accept(i, int(row[r]))
+                waited += 1
+        finally:
+            if begun:
+                eng.gen_end()
+            if cascade is not None:
+                eng.set_option("cascade_attn", cascade)
+            if procs.proc is not None:
+                eng.set_processors(None)
+        for i in rows:
+            if i is not None:
+                rq.end(i)
+
+    def _stop(self, i: int, finished: List[int]):
+        """request i is complete: release its slot (and what the caller keeps for it) and queue it for the next yield"""
+        if i in self.slots:
+            self.model.engine.seq_free(self.slots.pop(i))
+        self.release(i)
+        self.rq.end(i)
+        finished.append(i)
 
 
 class DetikzifyForCausalLM:
@@ -377,18 +512,6 @@ class DetikzifyForCausalLM:
             raise ValueError("The image patch tokens should be consecutive.")
         return st, n
 
-    @staticmethod
-    def _shared_prefix(prompts: Sequence[List[int]], lim: int, span: Tuple[int, int]) -> int:
-        """Longest common token prefix of the prompts, at most ``lim`` long; never splits the image span ``span`` of prompt 0
-        and is 0 below 16 positions (a shorter shared prefix saves less than the sharing costs)."""
-        lcp = 0
-        while lcp < lim and all(p[lcp] == prompts[0][lcp] for p in prompts[1:]):
-            lcp += 1
-        st0, n0 = span
-        if n0 and st0 < lcp < st0 + n0:
-            lcp = st0
-        return lcp if lcp >= 16 else 0
-
     def _batch_captions(self, adapter_input_ids, adapter_attention_mask, pixel_values, N: int):
         """TikZero captions of an N-sequence call (one shared or one per sequence) and the pixels to condition: a caption
         without an image runs on the adapter's dummy image."""
@@ -433,137 +556,10 @@ class DetikzifyForCausalLM:
             kv.tokens = []
             return kv.slot, False
 
-    # ---- generate --------------------------------------------------------------------------------
-    @torch.no_grad()
-    def generate(self, input_ids: torch.Tensor = None, pixel_values: Optional[torch.Tensor] = None,
-                 bad_words_ids=None, begin_suppress_tokens=None, streamer=None, stopping_criteria=None,
-                 temperature: Optional[float] = None, top_p: Optional[float] = None, top_k: Optional[int] = None,
-                 max_length: Optional[int] = None, max_new_tokens: Optional[int] = None,
-                 do_sample: Optional[bool] = None, seed: Optional[int] = None, eos_token_id: Optional[int] = None,
-                 adapter_input_ids=None, adapter_attention_mask=None, **ignored) -> torch.Tensor:
-        cfg, eng = self.config, self.engine
-        caption = None
-        if adapter_input_ids is not None:
-            caps = self._captions(adapter_input_ids, adapter_attention_mask)
-            if len(caps) != 1:
-                raise ValueError("generate() is batch-1: pass one caption")
-            caption = caps[0]
-            if pixel_values is None:
-                pixel_values = self.adapter.dummy_pixels()
-        gc = self.generation_config
-        temperature = gc.temperature if temperature is None else temperature
-        top_p = gc.top_p if top_p is None else top_p
-        top_k = gc.top_k if top_k is None else top_k
-        do_sample = gc.do_sample if do_sample is None else do_sample
-        eos = cfg.eos_token_id if eos_token_id is None else eos_token_id
-        procs = self._processors(bad_words_ids, begin_suppress_tokens, ignored, eos,
-                                 bool(do_sample) and float(temperature) >= 1e-5)
-
-        ids2d = input_ids if input_ids.dim() == 2 else input_ids[None]
-        if ids2d.shape[0] != 1:
-            raise ValueError("generate() is batch-1 (use generate_batch for parallel rollouts)")
-        ids_host: List[int] = ids2d[0].tolist()
-        T0 = len(ids_host)
-        if max_length is None:
-            max_length = T0 + max_new_tokens if max_new_tokens is not None else gc.max_length
-        max_length = min(int(max_length), eng.max_len)
-        criteria = StoppingCriteriaList(stopping_criteria or [])
-
-        with self._lock, self._on_stream():
-            # -- splice validation (v1/modeling_detikzify.py:176-184)
-            img, img_start = None, 0
-            patch = cfg.image_token_id
-            n_patch_tokens = ids_host.count(patch)
-            if pixel_values is not None and n_patch_tokens > 0:
-                if n_patch_tokens != cfg.num_patches:
-                    raise ValueError("The number of image patch tokens should be the same as the number of image patches.")
-                img_start = ids_host.index(patch)
-                if ids_host[img_start: img_start + n_patch_tokens] != [patch] * n_patch_tokens:
-                    raise ValueError("The image patch tokens should be consecutive.")
-                img = self._image_embeds(pixel_values, caption)
-            elif pixel_values is None and n_patch_tokens:
-                # patch tokens without an image: their KV comes from plain embeddings. Forget the image identity too, so a
-                # later call WITH the same image re-validates nothing against these slots (ADVICE r1)
-                self._img_cache = None
-                self._slot_tokens = []
-            if T0 == 0:
-                raise ValueError("empty prompt")
-            if streamer is not None:
-                streamer.put(ids2d.cpu())
-            if T0 >= max_length:
-                if streamer is not None:
-                    streamer.end()
-                return ids2d.to(self.device)
-
-            # -- longest common prefix with the KV already held by one of the cache slots
-            L = self._pick_slot(ids_host, img_start, n_patch_tokens if img is not None else 0)
-            ids_dev = torch.tensor(ids_host[L:], dtype=torch.int64)
-            if self.device.type == "cuda":
-                ids_dev = ids_dev.pin_memory().to(self.device, non_blocking=True)
-            self._slot_tokens = list(ids_host[:L])     # if the prefill raises, the slot only claims what it held before
-            last_logits, _ = eng.prefill(self._slot, ids_dev, L, img, img_start)
-            self._slot_tokens = list(ids_host)
-
-            self._call_counter += 1
-            params = eng.sampling(
-                temperature=temperature, top_p=top_p, top_k=top_k or 0, do_sample=bool(do_sample),
-                bad_token=procs.bad_token, begin_suppress_token=procs.bs_token,
-                seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
-            eos_min = [procs.eos_min(T0)]
-            if procs.proc is not None:
-                eng.set_processors(procs.proc, [ids_host], eos_min)
-            try:
-                first, _ = eng.sample(last_logits, params, suppress=[1], steps=[0])
-            except BaseException:
-                if procs.proc is not None:
-                    eng.set_processors(None)
-                raise
-            tok = int(first.item())
-
-            out_buf = torch.empty(1, max_length, dtype=torch.int64)
-            out_buf[0, :T0] = ids2d[0].cpu()
-            n_new = max_length - T0        # upper bound on new tokens
-            new_tokens: List[int] = []
-            launched = waited = 0
-            started = False
-            try:
-                while True:
-                    new_tokens.append(tok)
-                    out_buf[0, T0 + len(new_tokens) - 1] = tok
-                    if streamer is not None:
-                        streamer.put(out_buf[0, T0 + len(new_tokens) - 1: T0 + len(new_tokens)])
-                    cur = out_buf[:, : T0 + len(new_tokens)]
-                    if tok == eos or len(new_tokens) >= n_new or criteria(cur, None):
-                        break
-                    if not started:
-                        if procs.proc is not None:   # the device history continues from prompt + the first new token
-                            eng.set_processors(procs.proc, [ids_host + new_tokens], eos_min)
-                        eng.gen_begin([self._slot], [T0], [tok], params)
-                        started = True
-                    while launched < waited + 2 and launched < n_new - 1:
-                        eng.gen_step()
-                        launched += 1
-                    tok = eng.gen_wait(waited)[0]
-                    waited += 1
-            finally:
-                if started:
-                    eng.gen_end()
-                if procs.proc is not None:
-                    eng.set_processors(None)
-                # decode step s wrote KV at T0+s for new_tokens[s]; only tokens the host has seen count
-                self._slot_tokens = list(ids_host) + new_tokens[: min(launched, len(new_tokens))]
-            # exceptions escape before this point (the caller's error_callback feeds the streamer,
-            # detikzify/infer/generate.py:252); the normal path always terminates the stream
-            if streamer is not None:
-                streamer.end()
-            result = out_buf[:, : T0 + len(new_tokens)].to(self.device)
-            self._sync()
-            return result
-
-    # ---- batched generation (extension; the reference's generate() is batch-1) ---------------------
-    def _batch_sampling(self, temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
-                        kw: Dict[str, Any]) -> SimpleNamespace:
-        """The sampling and processor kwargs of a batched call, each falling back to ``generation_config``."""
+    # ---- generation: sampling kwargs, shared-prefix prefill, the three entry points ------------------------------
+    def _sampling(self, temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
+                  kw: Dict[str, Any]) -> SimpleNamespace:
+        """The sampling and processor kwargs of a generate call, each falling back to ``generation_config``."""
         gc = self.generation_config
         g = SimpleNamespace(temperature=gc.temperature if temperature is None else temperature,
                             top_p=gc.top_p if top_p is None else top_p, top_k=gc.top_k if top_k is None else top_k,
@@ -573,15 +569,55 @@ class DetikzifyForCausalLM:
                                    bool(g.do_sample) and float(g.temperature) >= 1e-5)
         return g
 
-    def _batch_params(self, g: SimpleNamespace, seed: Optional[int]):
+    def _sampling_params(self, g: SimpleNamespace, seed: Optional[int]):
+        """The engine's sampling parameters of one call; without ``seed`` every call draws from a new seed."""
         self._call_counter += 1
         return self.engine.sampling(
             temperature=g.temperature, top_p=g.top_p, top_k=g.top_k or 0, do_sample=bool(g.do_sample),
             bad_token=g.procs.bad_token, begin_suppress_token=g.procs.bs_token,
             seed=(seed if seed is not None else torch.initial_seed() + self._call_counter))
 
-    def _batch_requests(self, prompts: List[List[int]], streamers, stopping_criteria, max_length, max_new_tokens,
-                        eos: int) -> _Requests:
+    def _base_prefix(self, prompts: List[List[int]], span: Tuple[int, int], image,
+                     lim: Optional[int] = None) -> Tuple[Optional[int], int]:
+        """Prefill the longest common token prefix of the prompts of one image once into a new base slot: at most ``lim``
+        long (default: one short of the shortest prompt), never splitting prompt 0's image span ``span`` (``image()``: its
+        embeddings). Returns (base slot, shared length), or (None, 0) below 16 positions (a shorter shared prefix saves
+        less than the sharing costs), for a single prompt, or when no slot is free."""
+        eng = self.engine
+        if len(prompts) < 2:
+            return None, 0
+        lim = min(len(p) for p in prompts) - 1 if lim is None else lim
+        lcp = 0
+        while lcp < lim and all(p[lcp] == prompts[0][lcp] for p in prompts[1:]):
+            lcp += 1
+        st0, n0 = span
+        if n0 and st0 < lcp < st0 + n0:
+            lcp = st0
+        if lcp < 16:
+            return None, 0
+        try:
+            base = eng.seq_alloc()
+        except Exception:       # no spare slot: every sequence prefills its whole prompt
+            return None, 0
+        try:
+            eng.prefill(base, self._to_device_ids(prompts[0][:lcp]), 0, image() if n0 and st0 < lcp else None, st0)
+        except BaseException:
+            eng.seq_free(base)
+            raise
+        return base, lcp
+
+    def _prefill_row(self, slot: int, prompt: List[int], base: Optional[int], lcp: int, span: Tuple[int, int],
+                     image) -> torch.Tensor:
+        """``prompt`` into ``slot``, borrowing its first ``lcp`` positions from ``base``; the last position's logits."""
+        st, n = span
+        img = image() if n and st >= lcp else None
+        if lcp:
+            self.engine.seq_share(base, slot, lcp)
+        lg, _ = self.engine.prefill(slot, self._to_device_ids(prompt[lcp:]), lcp, img, st)
+        return lg
+
+    def _requests(self, prompts: List[List[int]], streamers, stopping_criteria, max_length, max_new_tokens,
+                  eos: int) -> _Requests:
         """Per-sequence streamers (one entry or None each), stopping criteria (a callable or list per sequence, or one shared
         entry) and ``max_length`` limits of N prompts."""
         N, gc = len(prompts), self.generation_config
@@ -600,6 +636,66 @@ class DetikzifyForCausalLM:
             limits.append(min(int(ml), self.engine.max_len))
         return _Requests(prompts, streamers, crits, limits, eos)
 
+    @torch.no_grad()
+    def generate(self, input_ids: torch.Tensor = None, pixel_values: Optional[torch.Tensor] = None,
+                 bad_words_ids=None, begin_suppress_tokens=None, streamer=None, stopping_criteria=None,
+                 temperature: Optional[float] = None, top_p: Optional[float] = None, top_k: Optional[int] = None,
+                 max_length: Optional[int] = None, max_new_tokens: Optional[int] = None,
+                 do_sample: Optional[bool] = None, seed: Optional[int] = None, eos_token_id: Optional[int] = None,
+                 adapter_input_ids=None, adapter_attention_mask=None, **ignored) -> torch.Tensor:
+        cfg = self.config
+        caption = None
+        if adapter_input_ids is not None:
+            caps = self._captions(adapter_input_ids, adapter_attention_mask)
+            if len(caps) != 1:
+                raise ValueError("generate() is batch-1: pass one caption")
+            caption = caps[0]
+            if pixel_values is None:
+                pixel_values = self.adapter.dummy_pixels()
+        g = self._sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens, ignored)
+
+        ids2d = input_ids if input_ids.dim() == 2 else input_ids[None]
+        if ids2d.shape[0] != 1:
+            raise ValueError("generate() is batch-1 (use generate_batch for parallel rollouts)")
+        ids_host: List[int] = ids2d[0].tolist()
+        T0 = len(ids_host)
+        rq = self._requests([ids_host], [streamer], stopping_criteria, max_length, max_new_tokens, g.eos)
+
+        with self._lock, self._on_stream():
+            # -- splice validation (v1/modeling_detikzify.py:176-184)
+            img = None
+            img_start, n_patch = self._image_span(ids_host) if pixel_values is not None else (0, 0)
+            if n_patch:
+                img = self._image_embeds(pixel_values, caption)
+            elif pixel_values is None and cfg.image_token_id in ids_host:
+                # patch tokens without an image: their KV comes from plain embeddings. Forget the image identity too, so a
+                # later call WITH the same image re-validates nothing against these slots (ADVICE r1)
+                self._img_cache = None
+                self._slot_tokens = []
+            if T0 == 0:
+                raise ValueError("empty prompt")
+            rq.start(0)
+            if rq.done[0]:
+                rq.end(0)
+                return ids2d.to(self.device)
+
+            # -- longest common prefix with the KV already held by one of the cache slots
+            L = self._pick_slot(ids_host, img_start, n_patch)
+            self._slot_tokens = list(ids_host[:L])     # if the prefill raises, the slot only claims what it held before
+            last_logits, _ = self.engine.prefill(self._slot, self._to_device_ids(ids_host[L:]), L, img, img_start)
+            self._slot_tokens = list(ids_host)
+
+            loop = _DecodeLoop(self, rq, g, seed, {0: self._slot})
+            try:
+                list(loop.run([0], [last_logits]))
+            finally:
+                # decode step s wrote KV at T0+s for new token s; only tokens the host has seen count
+                self._slot_tokens = ids_host + rq.ids(0)[0, T0: T0 + loop.launched].tolist()
+            result = rq.ids(0).to(self.device)
+            self._sync()
+            return result
+
+    # ---- batched generation (extension; the reference's generate() is batch-1) ---------------------
     @torch.no_grad()
     def generate_batch(self, input_ids: Sequence[torch.Tensor], pixel_values: Optional[torch.Tensor] = None, *,
                        bad_words_ids=None, begin_suppress_tokens=None, temperature: Optional[float] = None,
@@ -624,9 +720,7 @@ class DetikzifyForCausalLM:
         each sequence prefills only its own suffix. Returns a list of 1-D id tensors (prompt included).
         N is bounded by the engine's ``max_batch`` and free KV slots (``load(..., max_seqs=, max_batch=)``)."""
         eng = self.engine
-        g = self._batch_sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
-                                 ignored)
-        procs = g.procs
+        g = self._sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens, ignored)
         prompts: List[List[int]] = [(p[0] if p.dim() == 2 else p).tolist() for p in input_ids]
         N = len(prompts)
         if N == 0:
@@ -634,86 +728,32 @@ class DetikzifyForCausalLM:
         captions, pixel_values = self._batch_captions(adapter_input_ids, adapter_attention_mask, pixel_values, N)
         if any(len(p) == 0 for p in prompts):
             raise ValueError("empty prompt")
-        rq = self._batch_requests(prompts, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
+        rq = self._requests(prompts, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
         with self._lock, self._on_stream():
             imgs = self._batch_image_embeds(pixel_values, captions, N)
-            for i, st in enumerate(rq.streamers):
-                if st is not None:
-                    st.put(torch.tensor([prompts[i]], dtype=torch.int64))
-            slots: List[int] = []
-            base_slot = None
-            procs_set = False
+            spans = [self._image_span(p) if imgs is not None else (0, 0) for p in prompts]
+            image = [lambda i=i: imgs[i if imgs.shape[0] == N else 0] for i in range(N)]
+            slots: Dict[int, int] = {}
+            base, lcp = None, 0
             try:
-                for _ in range(N):
-                    slots.append(eng.seq_alloc())
-                # longest common prefix of the prompts (never splitting an image span, never a whole prompt)
-                lcp = 0
-                one_image = imgs is None or imgs.shape[0] == 1
-                if share_prefix and N > 1 and one_image:
-                    lcp = self._shared_prefix(prompts, min(len(p) for p in prompts) - 1,
-                                              self._image_span(prompts[0]) if imgs is not None else (0, 0))
-                if lcp:
-                    try:
-                        base_slot = eng.seq_alloc()
-                    except Exception:       # no spare slot: every sequence prefills its whole prompt
-                        base_slot, lcp = None, 0
-                if lcp:
-                    st0, n0 = self._image_span(prompts[0]) if imgs is not None else (0, 0)
-                    head = self._to_device_ids(prompts[0][:lcp])
-                    eng.prefill(base_slot, head, 0, imgs[0] if (imgs is not None and n0 and st0 < lcp) else None, st0)
-                last = []
-                for i, ids_host in enumerate(prompts):
-                    img, img_start = None, 0
-                    if imgs is not None:
-                        img_start, n_patch = self._image_span(ids_host)
-                        if n_patch and img_start >= lcp:
-                            img = imgs[i if imgs.shape[0] == N else 0]
-                    if lcp:
-                        eng.seq_share(base_slot, slots[i], lcp)
-                    lg, _ = eng.prefill(slots[i], self._to_device_ids(ids_host[lcp:]), lcp, img, img_start)
-                    last.append(lg)
-                params = self._batch_params(g, seed)
-                seq_ids = list(range(N))
-                eos_min = [procs.eos_min(len(p)) for p in prompts]
-                if procs.proc is not None:
-                    procs_set = True
-                    eng.set_processors(procs.proc, prompts, eos_min)
-                first, _ = eng.sample(torch.stack(last), params, suppress=[1] * N, steps=[0] * N, seq_ids=seq_ids)
-                toks = [int(t) for t in first.tolist()]
                 for i in range(N):
-                    if not rq.done[i]:
-                        rq.accept(i, toks[i])
-                max_steps = max(lim - len(p) for p, lim in zip(prompts, rq.limits)) - 1
-                if not all(rq.done) and max_steps > 0:
-                    if procs.proc is not None:   # device histories continue from prompt + first token (at most max_len ids)
-                        eng.set_processors(procs.proc, [(p + [t])[:eng.max_len] for p, t in zip(prompts, toks)], eos_min)
-                    eng.gen_begin(slots, [len(p) for p in prompts], toks, params, seq_ids)
-                    launched = waited = 0
-                    try:
-                        while not all(rq.done) and waited < max_steps:
-                            while launched < waited + 2 and launched < max_steps:
-                                eng.gen_step()
-                                launched += 1
-                            row = eng.gen_wait(waited)
-                            waited += 1
-                            for i in range(N):
-                                if not rq.done[i]:          # finished sequences keep decoding on the device; the host ignores them
-                                    rq.accept(i, int(row[i]))
-                    finally:
-                        eng.gen_end()
-                for st in rq.streamers:
-                    if st is not None:
-                        st.end()
-                result = [torch.tensor(o, dtype=torch.int64, device=self.device) for o in rq.outs]
+                    rq.start(i)
+                for i in range(N):
+                    slots[i] = eng.seq_alloc()
+                # one shared image: its prompts' longest common prefix is prefilled once (never splitting an image span)
+                if share_prefix and (imgs is None or imgs.shape[0] == 1):
+                    base, lcp = self._base_prefix(prompts, spans[0], image[0])
+                last = [self._prefill_row(slots[i], prompts[i], base, lcp, spans[i], image[i])
+                        for i in range(N)]
+                list(_DecodeLoop(self, rq, g, seed, slots).run(list(range(N)), last))
+                result = [rq.ids(i)[0].to(self.device) for i in range(N)]
                 self._sync()
                 return result
             finally:
-                if procs_set:
-                    eng.set_processors(None)
-                for s in slots:
+                for s in slots.values():
                     eng.seq_free(s)
-                if base_slot is not None:
-                    eng.seq_free(base_slot)
+                if base is not None:
+                    eng.seq_free(base)
 
     # ---- continuous batching (extension): a stream of requests through one running decode loop ---------
     def generate_many(self, prompts: Sequence[torch.Tensor], pixel_values: Optional[torch.Tensor] = None, *,
@@ -745,8 +785,7 @@ class DetikzifyForCausalLM:
         B = eng.max_batch if batch_size is None else int(batch_size)
         if not 2 <= B <= eng.max_batch:
             raise ValueError(f"batch_size must lie in [2, max_batch = {eng.max_batch}], got {batch_size!r}")
-        g = self._batch_sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens,
-                                 ignored)
+        g = self._sampling(temperature, top_p, top_k, do_sample, eos_token_id, bad_words_ids, begin_suppress_tokens, ignored)
         ids: List[List[int]] = [torch.as_tensor(p).reshape(-1).tolist() for p in prompts]
         N = len(ids)
         if any(len(p) == 0 for p in ids):
@@ -762,12 +801,12 @@ class DetikzifyForCausalLM:
         figure = [int(f) for f in figure]
         if len(figure) != N or any(not 0 <= f < F for f in figure):
             raise ValueError(f"figure must hold one index in [0, {F}) per prompt")
-        rq = self._batch_requests(ids, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
+        rq = self._requests(ids, streamers, stopping_criteria, max_length, max_new_tokens, g.eos)
         return self._many(ids, pix, figure, B, g, seed, rq)
 
     def _many(self, prompts: List[List[int]], pix: Optional[torch.Tensor], figure: List[int], B: int, g: SimpleNamespace,
               seed: Optional[int], rq: _Requests) -> Iterator[Tuple[int, torch.Tensor]]:
-        eng, procs, N = self.engine, g.procs, len(prompts)
+        eng, N = self.engine, len(prompts)
         spans = [self._image_span(p) if pix is not None else (0, 0) for p in prompts]
         members: Dict[int, List[int]] = {}
         for i, f in enumerate(figure):
@@ -777,10 +816,6 @@ class DetikzifyForCausalLM:
         embeds: Dict[int, torch.Tensor] = {}
         queue = deque(range(N))
         slot_of: Dict[int, int] = {}
-        rows: List[Optional[int]] = []       # occupant of each loop row (None = retired)
-        s0: List[int] = []                   # step from which the ring's entry of a row belongs to its occupant
-        finished: List[Tuple[int, torch.Tensor]] = []
-        state = dict(begun=False, procs=False, cascade=None)
 
         def figure_embeds(f: int) -> torch.Tensor:
             if f not in embeds:                                # the tower runs for the next figures in queue order
@@ -791,38 +826,17 @@ class DetikzifyForCausalLM:
                     embeds[h] = out[k]
             return embeds[f]
 
-        def figure_prefix(f: int) -> Tuple[Optional[int], int]:
-            if f not in bases:
-                ps = [prompts[i] for i in members[f]]
-                lcp = self._shared_prefix(ps, min(len(p) for p in ps) - 1, spans[members[f][0]]) if len(ps) > 1 else 0
-                base = None
-                if lcp:
-                    try:
-                        base = eng.seq_alloc()
-                    except Exception:       # no spare slot: the figure's sequences prefill their whole prompts
-                        lcp = 0
-                if lcp:
-                    st0, n0 = spans[members[f][0]]
-                    img = figure_embeds(f) if (pix is not None and n0 and st0 < lcp) else None
-                    eng.prefill(base, self._to_device_ids(prompts[members[f][0]][:lcp]), 0, img, st0)
-                bases[f] = (base, lcp)
-            return bases[f]
-
         def prefill(i: int, slot: int) -> torch.Tensor:
-            """prompt i into its slot after the figure's shared prefix; the last position's logits"""
+            """prompt i into its slot after its figure's shared prefix; the last position's logits"""
             f = figure[i]
-            base, lcp = figure_prefix(f)
-            img_start, n_patch = spans[i]
-            img = figure_embeds(f) if (pix is not None and n_patch and img_start >= lcp) else None
-            if lcp:
-                eng.seq_share(base, slot, lcp)
-            lg, _ = eng.prefill(slot, self._to_device_ids(prompts[i][lcp:]), lcp, img, img_start)
-            return lg
+            if f not in bases:
+                bases[f] = self._base_prefix([prompts[j] for j in members[f]], spans[members[f][0]],
+                                             lambda: figure_embeds(f))
+            base, lcp = bases[f]
+            return self._prefill_row(slot, prompts[i], base, lcp, spans[i], lambda: figure_embeds(f))
 
-        def stop(i: int):
-            """sequence i is complete: release its slot (and its figure's base after the last one) and queue its result"""
-            if i in slot_of:
-                eng.seq_free(slot_of.pop(i))
+        def release(i: int):
+            """after the figure's last sequence: its base slot and embeddings"""
             f = figure[i]
             left[f] -= 1
             if left[f] == 0:
@@ -830,17 +844,11 @@ class DetikzifyForCausalLM:
                 if base is not None:
                     eng.seq_free(base)
                 embeds.pop(f, None)
-            if rq.streamers[i] is not None:
-                rq.streamers[i].end()
-            finished.append((i, torch.tensor(rq.outs[i], dtype=torch.int64)))
-
-        def put_prompt(i: int):
-            if rq.streamers[i] is not None:
-                rq.streamers[i].put(torch.tensor([prompts[i]], dtype=torch.int64))
 
         self._lock.acquire()
         ctx = self._on_stream()
         ctx.__enter__()
+        run = None
         try:
             # ---- first wave: exactly generate_batch's calls for the first batch_size prompts
             wave = [queue.popleft() for _ in range(min(B, N))]
@@ -848,98 +856,24 @@ class DetikzifyForCausalLM:
                 for f in dict.fromkeys(figure[i] for i in wave):
                     figure_embeds(f)
             for i in wave:
-                put_prompt(i)
+                rq.start(i)
             for i in wave:
                 slot_of[i] = eng.seq_alloc()
             last = [prefill(i, slot_of[i]) for i in wave]
-            params = self._batch_params(g, seed)
-            eos_min = [procs.eos_min(len(prompts[i])) for i in wave]
-            if procs.proc is not None:
-                state["procs"] = True
-                eng.set_processors(procs.proc, [prompts[i] for i in wave], eos_min)
-            first, _ = eng.sample(torch.stack(last), params, suppress=[1] * len(wave), steps=[0] * len(wave), seq_ids=wave)
-            toks = [int(t) for t in first.tolist()]
-            for i, t in zip(wave, toks):
-                if not rq.done[i]:
-                    rq.accept(i, t)
-            # steps the admitted sequences can use at most (a sequence admitted at step s0 takes its last token from step
-            # s0 + limit - len(prompt) - 2); as in generate_batch, no step is launched beyond the longest of them
-            cap = max(rq.limits[i] - len(prompts[i]) for i in wave) - 1
-            if (not all(rq.done[i] for i in wave) and cap > 0) or queue:
-                if procs.proc is not None:
-                    eng.set_processors(procs.proc, [(prompts[i] + [t])[:eng.max_len] for i, t in zip(wave, toks)], eos_min)
-                if len(members) > 1 and state["cascade"] is None:   # one shared prefix per figure: per-row reads only
-                    state["cascade"] = eng.get_option("cascade_attn")
-                    eng.set_option("cascade_attn", 0)
-                eng.gen_begin([slot_of[i] for i in wave], [len(prompts[i]) for i in wave], toks, params, wave)
-                state["begun"] = True
-                rows, s0 = list(wave), [0] * len(wave)
-            launched = waited = 0
-            pending: List[int] = []              # rows admitted since the last step launch: first token not read yet
-            while True:
-                for r, i in enumerate(rows):
-                    if i is not None and rq.done[i]:
-                        eng.gen_retire(r)
-                        rows[r] = None
-                        stop(i)
-                if not state["begun"]:
-                    for i in wave:
-                        stop(i)
-                # admissions into free rows; a prompt already at its limit completes without one
-                for r in range(len(rows)):
-                    while rows[r] is None and queue:
-                        i = queue[0]
-                        if rq.done[i]:
-                            queue.popleft()
-                            put_prompt(i)
-                            stop(i)
-                            continue
-                        try:
-                            slot = eng.seq_alloc()
-                        except Exception:
-                            if any(o is not None for o in rows):
-                                break               # wait for a slot to be released
-                            raise
-                        queue.popleft()
-                        slot_of[i] = slot
-                        put_prompt(i)
-                        lg = prefill(i, slot)
-                        eng.gen_admit(r, slot, len(prompts[i]), lg, i,
-                                      prompts[i] if procs.proc is not None else None, procs.eos_min(len(prompts[i])))
-                        rows[r], s0[r] = i, launched
-                        cap = max(cap, launched + rq.limits[i] - len(prompts[i]) - 1)
-                        pending.append(r)
-                if finished:
-                    out, finished[:] = list(finished), []
-                    ctx.__exit__(None, None, None)
-                    try:
-                        yield from out
-                    finally:
-                        ctx = self._on_stream()
-                        ctx.__enter__()
-                if all(i is None for i in rows):
-                    break
-                while launched < waited + 2 and launched < cap:
-                    eng.gen_step()
-                    launched += 1
-                for r in pending:                    # the admission kernels ran before the steps just launched
-                    rq.accept(rows[r], eng.gen_first(r))
-                pending = []
-                if not any(i is not None and not rq.done[i] for i in rows):
-                    continue
-                row = eng.gen_wait(waited)
-                for r, i in enumerate(rows):
-                    if i is not None and waited >= s0[r] and not rq.done[i]:
-                        rq.accept(i, int(row[r]))
-                waited += 1
+            # one shared prefix per figure: per-row reads only
+            loop = _DecodeLoop(self, rq, g, seed, slot_of, queue, prefill, release, per_row_attn=len(members) > 1)
+            run = loop.run(wave, last)
+            for done in run:
+                ctx.__exit__(None, None, None)
+                try:
+                    yield from ((i, rq.ids(i)[0].clone()) for i in done)
+                finally:
+                    ctx = self._on_stream()
+                    ctx.__enter__()
         finally:
             try:
-                if state["begun"]:
-                    eng.gen_end()
-                if state["cascade"] is not None:
-                    eng.set_option("cascade_attn", state["cascade"])
-                if state["procs"]:
-                    eng.set_processors(None)
+                if run is not None:
+                    run.close()      # the loop ends before the slots it reads are freed
                 for slot in slot_of.values():
                     eng.seq_free(slot)
                 for base, _ in bases.values():
@@ -1066,21 +1000,11 @@ class DetikzifyForCausalLM:
         with self._lock, self._on_stream():
             imgs = self._batch_image_embeds(pixel_values, captions, N)
             spans = [self._image_span(q) if imgs is not None else (0, 0) for q in seqs]
-            lcp = 0
-            if N > 1 and (imgs is None or imgs.shape[0] == 1):
-                lcp = self._shared_prefix(seqs, min(starts), spans[0])
             work, owned = self._scratch_slot()
-            base = None
+            base, lcp = None, 0
             try:
-                if lcp:
-                    try:
-                        base = eng.seq_alloc()
-                    except Exception:       # no spare slot (the working slot was borrowed too): no sharing
-                        lcp = 0
-                if lcp:
-                    st0, n0 = spans[0]
-                    eng.prefill(base, self._to_device_ids(seqs[0][:lcp]), 0,
-                                imgs[0] if (imgs is not None and n0 and st0 < lcp) else None, st0)
+                if imgs is None or imgs.shape[0] == 1:
+                    base, lcp = self._base_prefix(seqs, spans[0], lambda: imgs[0], lim=min(starts))
                 out = []
                 for i, q in enumerate(seqs):
                     s0 = min(lcp, starts[i] - 1)              # positions borrowed from the base slot
