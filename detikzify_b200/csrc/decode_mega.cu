@@ -504,6 +504,7 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
   asm volatile("setmaxnreg.inc.sync.aligned.u32 224;\n");
   const int dflags = DBG ? p.dbg_flags : 0;
   const bool nowait = (dflags & 2) != 0;
+  const int stage_pass = (p.variant & 2) ? 0 : 1;   // weight tiles: stage the input slice before (0) or after (1) reading the tile
   unsigned long long bar_target = p.bar_base[0];   // arrivals counted before this launch
   const uint32_t epoch = (uint32_t)p.bar_base[1];  // tag of phase it = epoch + it + 1
   Walk w;
@@ -861,154 +862,124 @@ __global__ void __launch_bounds__(MEGA_THREADS, 1) decode_mega_kernel(const Mega
             if (row < 160u) trow = ctr + row * 4;
           }
           if (DBG && trow && lane == 0) trow[3] = clock64();
-          // the tile's slice of the input vector (normally staged by this very warp at its previous tile of the same ks)
-          if (*reinterpret_cast<volatile uint32_t*>(slice_tag + ks) != tag)
-            stage_slice(src, tag - 1, nowait, p.embed + (int64_t)tok * p.H, K, (int)ks, nw, xb, slice_ss, slice_tag, tag);
-          mbar_wait(full0 + 8 * sl, use & 1);
-          if (DBG && trow && lane == 0) trow[1] = clock64();
-          // ---- one tile = 16 k-steps of (ldmatrix.x4, mma). B operand: even columns of the 16 x 8 B tile carry the hi
-          // part of x, odd columns the lo part (column = lane >> 2), so ONE mma per k-step yields W.hi in accumulator
-          // column 0 and W.lo in column 1. The A fragments are loaded in batches interleaved with the mma of earlier
-          // batches, so that the tensor pipe starts while the rest of the tile is still being read (shared-memory returns
-          // are in order; all 16 ldmatrix in front of the first mma make the two pipes take turns).
-          float rA0, rA2;
-          if (F8 && ph != PH_LM) {
-            // ---- e4m3 tile: [kstep pair][lane][16 B] = this lane's A fragments of two k-steps, converted in registers to the
-            // bf16 bits of code x 2^k_r (rows g and g + 8 of the group: one scale each); same mma sequence as the bf16 tile
+          // ---- one tile = 16 k-steps of mma.m16n8k16. The warp first waits for the tile, reads it and hands the slot back,
+          // rebuilds the A fragments of all 16 k-steps in registers (ldmatrix for bf16 tiles; the FP8 or packed conversion),
+          // and only then stages the tile's slice of the input vector if it is not staged yet (normally this very warp staged
+          // it at its previous tile of the same ks; at the warp's first tile of a phase the staging polls the previous phase's
+          // output, the cross-CTA hop). So the slot is free for the producer during the hop and the conversion runs while the
+          // warp would otherwise wait for its input: after the hop only the B loads and the mma chain remain.
+          // (mega_variant bit 1: stage first, as earlier builds did; the same results, for A/B runs.)
+          uint32_t A[16][4];
+#pragma unroll 1
+          for (int pass = 0; pass < 2; ++pass) {
+            if (pass == stage_pass && *reinterpret_cast<volatile uint32_t*>(slice_tag + ks) != tag)
+              stage_slice(src, tag - 1, nowait, p.embed + (int64_t)tok * p.H, K, (int)ks, nw, xb, slice_ss, slice_tag, tag);
+            if (pass == 1) break;
+            mbar_wait(full0 + 8 * sl, use & 1);
+            if (DBG && trow && lane == 0) trow[1] = clock64();
             cur_slot = sl;
-            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
-            const uint32_t ta = ring_u32 + sl * TILE_BYTES + lane * 16;
-            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
-            uint2 b[16];
-#pragma unroll
-            for (int s = 0; s < 16; ++s) b[s] = xp[s * 8];
-            uint4 q[8];
-#pragma unroll
-            for (int s = 0; s < 8; ++s)
-              asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[s].x), "=r"(q[s].y), "=r"(q[s].z), "=r"(q[s].w) : "r"(ta + s * 512));
-            int e0, e1;
-            {
-              const uint32_t ea = ring_u32 + sl * TILE_BYTES + MEGA_F8_TILE_BYTES + (lane >> 2);
-              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e0) : "r"(ea));
-              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e1) : "r"(ea + 8));
-            }
-            release();
-            const float s0 = pow2f(e0), s1 = pow2f(e1);
-            if (!(dflags & 1)) {
-#pragma unroll
-              for (int s = 0; s < 8; ++s) {
-                const uint32_t a0[4] = {e4m3x2_to_bf16x2(q[s].x, s0), e4m3x2_to_bf16x2(q[s].x >> 16, s1),
-                                        e4m3x2_to_bf16x2(q[s].y, s0), e4m3x2_to_bf16x2(q[s].y >> 16, s1)};
-                const uint32_t a1[4] = {e4m3x2_to_bf16x2(q[s].z, s0), e4m3x2_to_bf16x2(q[s].z >> 16, s1),
-                                        e4m3x2_to_bf16x2(q[s].w, s0), e4m3x2_to_bf16x2(q[s].w >> 16, s1)};
-                mma_bf16_16816(acc, a0, b[2 * s].x, b[2 * s].y);
-                mma_bf16_16816(c1, a1, b[2 * s + 1].x, b[2 * s + 1].y);
-              }
-            }
-            rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);
-            rA2 = (acc[2] + c1[2]) + (acc[3] + c1[3]);
-          } else if (PK) {
-            // ---- packed tile (MegaPack): one pair of an A fragment = two bytes sign | mantissa7 (word w of the byte plane, the
-            // same order as the e4m3 codes) and two exponent bytes (cb, the matching word of exponent codes, or of biased
-            // exponents in an escape tile): prmt spreads the bytes into the bf16 halves (the sign replicated up to bit 15),
-            // the codes go to bits 7..11 and the row base is added there. Rows g and g + 8 of the group: one base each.
-            cur_slot = sl;
-            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
             const uint32_t tb = ring_u32 + sl * TILE_BYTES;
-            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
-            uint4 q[8], nb[4], hb;
-            // the tile is read in two halves of 4 kstep pairs (bytes and codes), the slot handed back after the second: the first
-            // half's mma run while the second half is still in flight, and the A operands of 8 ksteps are live at a time
-            auto ld_half = [&](int h) {
+            if (F8 && ph != PH_LM) {
+              // ---- e4m3 tile: [kstep pair][lane][16 B] = this lane's A fragments of two k-steps, converted in registers to the
+              // bf16 bits of code x 2^k_r (rows g and g + 8 of the group: one scale each)
+              uint4 q[8];
 #pragma unroll
-              for (int s = 4 * h; s < 4 * h + 4; ++s)
+              for (int s = 0; s < 8; ++s)
                 asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[s].x), "=r"(q[s].y), "=r"(q[s].z), "=r"(q[s].w) : "r"(tb + lane * 16 + s * 512));
-#pragma unroll
-              for (int s = 2 * h; s < 2 * h + 2; ++s)
-                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(nb[s].x), "=r"(nb[s].y), "=r"(nb[s].z), "=r"(nb[s].w) : "r"(tb + MEGA_PK_NIB + lane * 16 + s * 512));
-            };
-            ld_half(0);
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(hb.x), "=r"(hb.y), "=r"(hb.z), "=r"(hb.w) : "r"(tb + MEGA_PK_HB + lane * 16));
-            uint32_t r0, r1;
-            int ei;
-            asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r0) : "r"(tb + MEGA_PK_HDR + (lane >> 2)));
-            asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r1) : "r"(tb + MEGA_PK_HDR + 8 + (lane >> 2)));
-            asm volatile("ld.shared.s32 %0, [%1];\n" : "=r"(ei) : "r"(tb + MEGA_PK_HDR + 16));
-            // kstep pairs [4 h, 4 h + 4); cbw(s): the exponent bytes of the 16 values of kstep pair s, one word per word of q[s]
-            auto tile_mma = [&](int h, uint32_t bb0, uint32_t bb1, auto&& cbw) {
-#pragma unroll
-              for (int s = 4 * h; s < 4 * h + 4; ++s) {
-                const uint4 cb = cbw(s);
-                const uint32_t w[4] = {q[s].x, q[s].y, q[s].z, q[s].w}, e[4] = {cb.x, cb.y, cb.z, cb.w};
-                uint32_t a[2][4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  uint32_t s0, s1;
-                  asm("prmt.b32 %0, %1, 0, 0x9180;\n" : "=r"(s0) : "r"(w[k]));
-                  asm("prmt.b32 %0, %1, 0, 0xB3A2;\n" : "=r"(s1) : "r"(w[k]));
-                  a[k >> 1][2 * (k & 1)] = (__byte_perm(e[k], 0u, 0x4140) << 7) + ((s0 & 0x807F807Fu) | bb0);
-                  a[k >> 1][2 * (k & 1) + 1] = (__byte_perm(e[k], 0u, 0x4342) << 7) + ((s1 & 0x807F807Fu) | bb1);
-                }
-                const uint2 b0 = xp[16 * s], b1 = xp[16 * s + 8];   // the input vector's B fragments of ksteps 2 s, 2 s + 1
-                mma_bf16_16816(acc, a[0], b0.x, b0.y);
-                mma_bf16_16816(c1, a[1], b1.x, b1.y);
-              }
-            };
-            // code of byte i of word k of kstep pair s: nibble i of nibble word k >> 1 (low / high half by k & 1), bit
-            // 8 i + 4 (s & 1) + k of high-bit word s >> 1; one lop3 merges them into a byte per value
-            auto codes = [&](int s) {
-              const uint32_t n0 = (s & 1) ? nb[s >> 1].z : nb[s >> 1].x, n1 = (s & 1) ? nb[s >> 1].w : nb[s >> 1].y;
-              const uint32_t hw = (s >> 1) == 0 ? hb.x : (s >> 1) == 1 ? hb.y : (s >> 1) == 2 ? hb.z : hb.w;
-              uint32_t cb[4];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const int t = 4 * (s & 1) + k;   // the code's high bit goes from bit 8 i + t to bit 8 i + 4
-                const uint32_t hs = t >= 4 ? hw >> (t - 4) : hw << (4 - t);
-                cb[k] = (((k >> 1) ? n1 : n0) >> (4 * (k & 1)) & 0x0F0F0F0Fu) | (hs & 0x10101010u);
-              }
-              return make_uint4(cb[0], cb[1], cb[2], cb[3]);
-            };
-            // escape tile: the biased exponents themselves, from the side buffer (base 0)
-            const uint4* ep = reinterpret_cast<const uint4*>(p.pk_esc + (int64_t)(ei < 0 ? 0 : ei) * MEGA_PK_ESC_BYTES) + lane;
-            auto escaped = [&](int s) { return __ldg(ep + s * 32); };
-            const uint32_t bb0 = r0 * 0x00800080u, bb1 = r1 * 0x00800080u;   // row base at bits 7 and 23
-            if (!(dflags & 1)) {
-              if (ei < 0) tile_mma(0, bb0, bb1, codes);
-              else tile_mma(0, 0u, 0u, escaped);
-            }
-            ld_half(1);
-            release();
-            if (!(dflags & 1)) {
-              if (ei < 0) tile_mma(1, bb0, bb1, codes);
-              else tile_mma(1, 0u, 0u, escaped);
-            }
-            rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);
-            rA2 = (acc[2] + c1[2]) + (acc[3] + c1[3]);
-          } else {
-            cur_slot = sl;
-            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
-            const uint32_t ta = ring_u32 + sl * TILE_BYTES + lane * 16;
-            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
-            uint2 b[16];
-#pragma unroll
-            for (int s = 0; s < 16; ++s) b[s] = xp[s * 8];
-            uint32_t a[16][4];
-#pragma unroll
-            for (int s = 0; s < 8; ++s) ldmatrix_x4(a[s][0], a[s][1], a[s][2], a[s][3], ta + s * 512);
-#pragma unroll
-            for (int bq = 0; bq < 4; ++bq) {
-              if (bq < 2) {
-#pragma unroll
-                for (int s = 8 + 4 * bq; s < 12 + 4 * bq; ++s) ldmatrix_x4(a[s][0], a[s][1], a[s][2], a[s][3], ta + s * 512);
-              }
-              if (bq == 1) release();
+              int e0, e1;
+              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e0) : "r"(tb + MEGA_F8_TILE_BYTES + (lane >> 2)));
+              asm volatile("ld.shared.s8 %0, [%1];\n" : "=r"(e1) : "r"(tb + MEGA_F8_TILE_BYTES + 8 + (lane >> 2)));
+              release();
+              const float s0 = pow2f(e0), s1 = pow2f(e1);
               if (!(dflags & 1)) {
 #pragma unroll
-                for (int s = 4 * bq; s < 4 * bq + 4; s += 2) {
-                  mma_bf16_16816(acc, a[s], b[s].x, b[s].y);
-                  mma_bf16_16816(c1, a[s + 1], b[s + 1].x, b[s + 1].y);
+                for (int s = 0; s < 8; ++s) {
+                  A[2 * s][0] = e4m3x2_to_bf16x2(q[s].x, s0);
+                  A[2 * s][1] = e4m3x2_to_bf16x2(q[s].x >> 16, s1);
+                  A[2 * s][2] = e4m3x2_to_bf16x2(q[s].y, s0);
+                  A[2 * s][3] = e4m3x2_to_bf16x2(q[s].y >> 16, s1);
+                  A[2 * s + 1][0] = e4m3x2_to_bf16x2(q[s].z, s0);
+                  A[2 * s + 1][1] = e4m3x2_to_bf16x2(q[s].z >> 16, s1);
+                  A[2 * s + 1][2] = e4m3x2_to_bf16x2(q[s].w, s0);
+                  A[2 * s + 1][3] = e4m3x2_to_bf16x2(q[s].w >> 16, s1);
                 }
               }
+            } else if (PK) {
+              // ---- packed tile (MegaPack): byte i of word k of kstep pair s is sign | mantissa7 of one value (the e4m3 codes'
+              // order: word k = kstep 2 s + (k >> 1), bytes 0-1 in row g, bytes 2-3 in row g + 8); its exponent is the row base
+              // plus a 5-bit code (nibble plane + high-bit plane), or in an escape tile the biased exponent itself (side buffer)
+              uint4 q[8], nb[4], hb;
+#pragma unroll
+              for (int s = 0; s < 8; ++s)
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(q[s].x), "=r"(q[s].y), "=r"(q[s].z), "=r"(q[s].w) : "r"(tb + lane * 16 + s * 512));
+#pragma unroll
+              for (int s = 0; s < 4; ++s)
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(nb[s].x), "=r"(nb[s].y), "=r"(nb[s].z), "=r"(nb[s].w) : "r"(tb + MEGA_PK_NIB + lane * 16 + s * 512));
+              asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(hb.x), "=r"(hb.y), "=r"(hb.z), "=r"(hb.w) : "r"(tb + MEGA_PK_HB + lane * 16));
+              uint32_t r0, r1;
+              int ei;
+              asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r0) : "r"(tb + MEGA_PK_HDR + (lane >> 2)));
+              asm volatile("ld.shared.u8 %0, [%1];\n" : "=r"(r1) : "r"(tb + MEGA_PK_HDR + 8 + (lane >> 2)));
+              asm volatile("ld.shared.s32 %0, [%1];\n" : "=r"(ei) : "r"(tb + MEGA_PK_HDR + 16));
+              release();
+              if (!(dflags & 1)) {
+                uint32_t ex[8][4];   // the exponent byte of every value, four per word of q
+                if (ei < 0) {
+                  // code of byte i of word k of kstep pair s: nibble i of nibble word k >> 1 (low / high half by k & 1), bit
+                  // 8 i + 4 (s & 1) + k of high-bit word s >> 1. Code <= 31 and base <= 224: one add for the four bytes (no carry)
+                  const uint32_t bb = r0 * 0x00000101u + r1 * 0x01010000u;
+#pragma unroll
+                  for (int s = 0; s < 8; ++s) {
+                    const uint32_t n0 = (s & 1) ? nb[s >> 1].z : nb[s >> 1].x, n1 = (s & 1) ? nb[s >> 1].w : nb[s >> 1].y;
+                    const uint32_t hw = (s >> 1) == 0 ? hb.x : (s >> 1) == 1 ? hb.y : (s >> 1) == 2 ? hb.z : hb.w;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                      const int t = 4 * (s & 1) + k;   // the code's high bit goes from bit 8 i + t to bit 8 i + 4
+                      const uint32_t hs = t >= 4 ? hw >> (t - 4) : hw << (4 - t);
+                      ex[s][k] = ((((k >> 1) ? n1 : n0) >> (4 * (k & 1)) & 0x0F0F0F0Fu) | (hs & 0x10101010u)) + bb;
+                    }
+                  }
+                } else {
+                  const uint4* ep = reinterpret_cast<const uint4*>(p.pk_esc + (int64_t)ei * MEGA_PK_ESC_BYTES) + lane;
+#pragma unroll
+                  for (int s = 0; s < 8; ++s) {
+                    const uint4 e = __ldg(ep + s * 32);
+                    ex[s][0] = e.x; ex[s][1] = e.y; ex[s][2] = e.z; ex[s][3] = e.w;
+                  }
+                }
+                // bf16 value = hi byte (sign | exponent >> 1) : lo byte (exponent bit 0 | mantissa7); two prmt interleave
+                // the four values' bytes into the A registers of rows g (bytes 0-1) and g + 8 (bytes 2-3)
+#pragma unroll
+                for (int s = 0; s < 8; ++s) {
+                  const uint32_t w[4] = {q[s].x, q[s].y, q[s].z, q[s].w};
+#pragma unroll
+                  for (int k = 0; k < 4; ++k) {
+                    uint32_t lo, hi;   // bit select (c ? a : b): one lop3 each
+                    asm("lop3.b32 %0, %1, %2, 0x7F7F7F7F, 0xE4;\n" : "=r"(lo) : "r"(w[k]), "r"(ex[s][k] << 7));
+                    asm("lop3.b32 %0, %1, %2, 0x80808080, 0xE4;\n" : "=r"(hi) : "r"(w[k]), "r"(ex[s][k] >> 1));
+                    uint32_t* a = A[2 * s + (k >> 1)] + 2 * (k & 1);
+                    asm("prmt.b32 %0, %1, %2, 0x5140;\n" : "=r"(a[0]) : "r"(lo), "r"(hi));
+                    asm("prmt.b32 %0, %1, %2, 0x7362;\n" : "=r"(a[1]) : "r"(lo), "r"(hi));
+                  }
+                }
+              }
+            } else {
+#pragma unroll
+              for (int s = 0; s < 16; ++s) ldmatrix_x4(A[s][0], A[s][1], A[s][2], A[s][3], tb + lane * 16 + s * 512);
+              release();
+            }
+          }
+          // B operand: even columns of the 16 x 8 B tile carry the hi part of x, odd columns the lo part (column = lane >> 2), so
+          // ONE mma per k-step yields W.hi in accumulator column 0 and W.lo in column 1; even k-steps go to acc, odd ones to c1
+          float rA0 = 0.f, rA2 = 0.f;
+          if (!(dflags & 1)) {
+            const uint2* xp = reinterpret_cast<const uint2*>(xb + (size_t)ks * 64 + (lane & 3)) + ((lane >> 2) & 1);
+            float acc[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+            for (int s = 0; s < 16; s += 2) {
+              const uint2 b0 = xp[8 * s], b1 = xp[8 * s + 8];
+              mma_bf16_16816(acc, A[s], b0.x, b0.y);
+              mma_bf16_16816(c1, A[s + 1], b1.x, b1.y);
             }
             // lanes with (lane & 3) == 0 hold columns 0 (hi) and 1 (lo) of rows g (c[0], c[1]) and g + 8 (c[2], c[3])
             rA0 = (acc[0] + c1[0]) + (acc[1] + c1[1]);

@@ -341,7 +341,7 @@ struct MegaArgs {
   unsigned long long* amax;                                   // [0] packed (ordered logit, ~index) max cell, [1] arrival counter; zero-initialised, self-resetting
   int *gen_tok, *gen_pos;
   unsigned long long *gen_step, *host_ring;
-  int variant;                                                // dev A/B switches (option "mega_variant"; results identical): bit 0 = weight copies without the evict_first L2 policy
+  int variant;                                                // dev A/B switches (option "mega_variant"; results identical): bit 0 = weight copies without the evict_first L2 policy, bit 1 = consumers stage a weight tile's input slice before reading the tile (earlier builds' order)
   int dbg_flags;                                              // dev only: 1 = skip tile math, 2 = skip grid barriers, 4/8 = relaxed arrive/poll
   long long* dbg;                                             // optional: [grid][5L+1][4] globaltimer stamps (null = off)
   long long* dbg2;                                            // optional: [grid][MEGA_DBG2_ROWS][4] clock64 per-tile trace of layer dbg_layer
