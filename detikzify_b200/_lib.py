@@ -101,6 +101,7 @@ SYMBOLS = {
     "dtk_dbg_mega_trace": (C.c_int, [_P, C.POINTER(C.c_longlong), C.c_int]),
     "dtk_dbg_pack_bytes": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
     "dtk_dbg_kv_read": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "dtk_dbg_residual_read": (C.c_int, [_P, C.c_int, C.c_int, _P, _P]),
     "dtk_dbg_gemm_impl": (C.c_int, [C.c_int]),
     "dtk_dbg_gemm": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "dtk_dbg_sample": (C.c_int, [_P, C.c_int, C.c_int, C.POINTER(DtkSampling), C.POINTER(C.c_int), C.POINTER(C.c_uint32),

@@ -283,6 +283,7 @@ struct dtk_engine {
   int fuse_greedy = 1;
   int cascade_attn = 1;      // batched decode: rows that share one prefix reduce it with ONE tensor-core pass (option "cascade_attn")
   int cas_slot = -1, cas_len = 0;   // set per step by dtk_decode / dtk_gen_begin: uniform shared prefix of the current batch
+  int prefill_layers = -1;   // dev option "prefill_layers": decoder_stack runs only the first n layers (-1 = all)
 
   // TikZero adapter (dtk_adapter_attach): borrowed arena, caption-encoder workspace (max_text rows) and the conditioned
   // ViT's caption buffers (one ViT chunk of captions)
@@ -1531,7 +1532,8 @@ int dtk_seq_share(dtk_engine* eng, int base, int dst, int len, void* stream) {
 
 namespace {
 // embedding splice + every decoder layer over ids[0..T) at positions [start_pos, start_pos + T) of `slot` (KV appended);
-// leaves the residual stream in p_x. Shared by dtk_prefill and dtk_score.
+// leaves the residual stream in p_x. Shared by dtk_prefill and dtk_score. The dev option "prefill_layers" = n stops the
+// stack after layer n (layers >= n write no KV rows).
 int decoder_stack(dtk_engine* eng, int slot, const int64_t* ids, int T, int start_pos, const float* img_embeds, int img_start,
                   int n_img, cudaStream_t s) {
   const dtk_config& c = eng->cfg;
@@ -1545,7 +1547,8 @@ int decoder_stack(dtk_engine* eng, int slot, const int64_t* ids, int T, int star
   const int H = c.hidden, I = c.inter, HD = c.head_dim, qd = c.heads * HD, kd = c.kv_heads * HD;
   DTK_CK(launch_embed_splice(ids, T, start_pos, W(eng, "dec.embed"), H, c.vocab, c.image_token_id, img_embeds, img_start,
                              n_img, eng->p_x, s, lc));
-  for (int l = 0; l < c.layers; ++l) {
+  const int layers = eng->prefill_layers >= 0 ? eng->prefill_layers : c.layers;
+  for (int l = 0; l < layers; ++l) {
     DTK_CK(launch_rmsnorm(eng->p_x, H, W(eng, LN("dec.L", l, "norm1")), c.rms_eps, T, H, eng->p_xn, s, lc));
     {
       GemmArgs g{};
@@ -2052,6 +2055,11 @@ int dtk_set_option(dtk_engine* eng, const char* key, int64_t value) {
     eng->mega_trace_layer = (int)value;
     return DTK_OK;
   }
+  if (std::strcmp(key, "prefill_layers") == 0) {  // dev: prefill / score run only the first n decoder layers (-1 = all)
+    DTK_REQUIRE(value >= -1 && value <= eng->cfg.layers, "prefill_layers must be in -1..layers");
+    eng->prefill_layers = (int)value;
+    return DTK_OK;
+  }
   eng->err = std::string("unknown option ") + key;
   return DTK_ERR_INVALID;
 }
@@ -2070,6 +2078,7 @@ int dtk_get_option(dtk_engine* eng, const char* key, int64_t* value) {
   if (std::strcmp(key, "decode_fp8") == 0) { *value = eng->decode_fp8; return DTK_OK; }
   if (std::strcmp(key, "decode_pack") == 0) { *value = eng->decode_pack; return DTK_OK; }
   if (std::strcmp(key, "decode_pack_escapes") == 0) { *value = eng->pk_escapes; return DTK_OK; }
+  if (std::strcmp(key, "prefill_layers") == 0) { *value = eng->prefill_layers; return DTK_OK; }
   if (std::strcmp(key, "decode_weight_bytes") == 0) {
     *value = (int64_t)(eng->decode_pack ? decode_pack_weight_bytes(eng) : decode_weight_bytes(eng->cfg, eng->decode_fp8 != 0));
     return DTK_OK;
@@ -2133,6 +2142,17 @@ int dtk_dbg_kv_read(dtk_engine* eng, int slot, int layer, int pos0, int n, void*
     DTK_CK(cudaMemcpy2DAsync(static_cast<bf16*>(v_out) + off, dst_pitch, k + eng->kv_v_offset, src_pitch, width, c.kv_heads,
                              cudaMemcpyDeviceToDevice, s));
   }
+  return DTK_OK;
+}
+
+int dtk_dbg_residual_read(dtk_engine* eng, int row0, int n, float* out, void* stream) {
+  if (!eng) return DTK_ERR_INVALID;
+  const dtk_config& c = eng->cfg;
+  DTK_REQUIRE(out, "null pointer");
+  DTK_REQUIRE(row0 >= 0 && n >= 0 && (int64_t)row0 + n <= c.max_len, "rows outside [0, max_len)");
+  DTK_CK(cudaSetDevice(eng->device));
+  DTK_CK(cudaMemcpyAsync(out, eng->p_x + (int64_t)row0 * c.hidden, (size_t)n * c.hidden * sizeof(float),
+                         cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return DTK_OK;
 }
 

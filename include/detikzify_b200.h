@@ -282,6 +282,9 @@ DTK_API int dtk_gen_first(dtk_engine* eng, int row, int32_t* token_out_host);
  *      mma.sync), "cascade_attn" (shared-prefix attention of batched decode), "decode_gemm_min_batch",
  *      "fuse_greedy", "vit_graph", and dev switches "mega_debug", "mega_flags", "mega_trace_layer",
  *      "mega_nslots", "mega_variant". Unknown keys return DTK_ERR_INVALID.
+ *      "prefill_layers" (dev switch for layer-by-layer tests): n in 0..layers makes dtk_prefill / dtk_score run only
+ *      the first n decoder layers; layers >= n write no KV rows and the logits come from the partial residual stream
+ *      (see dtk_dbg_residual_read). -1 (default) = every layer; other values return DTK_ERR_INVALID.
  *      "decode_fp8": 1 = the persistent kernel (B = 1) and the four layer GEMMs of batched steps with
  *      4 <= B < 64 stream the four decoder-layer matrices as e4m3 codes plus one power-of-two exponent per row
  *      (rebuilt from the arena, whose every row must be e4m3 x 2^k; otherwise DTK_ERR_INVALID names the layer
@@ -318,6 +321,10 @@ DTK_API int dtk_dbg_pack_bytes(dtk_engine* eng, int64_t offset, int64_t nbytes, 
  * of an allocated slot into k_out / v_out, each [kv_heads][n][head_dim]. Positions below the slot's shared length come from
  * the slot that lends them, as decode reads them. DTK_ERR_INVALID: slot not allocated, layer or range outside the cache. */
 DTK_API int dtk_dbg_kv_read(dtk_engine* eng, int slot, int layer, int pos0, int n, void* k_out, void* v_out, void* stream);
+/* copy (stream-ordered, no engine state changes) rows [row0, row0 + n) of the fp32 residual stream as the last dtk_prefill /
+ * dtk_score left it (row t = the t-th prompt position of that call) into out [n][hidden]. The contents are valid only until
+ * the next engine call. DTK_ERR_INVALID: null out, rows outside [0, max_len). */
+DTK_API int dtk_dbg_residual_read(dtk_engine* eng, int row0, int n, float* out, void* stream);
 /* select the dense GEMM implementation used by dtk_dbg_gemm and the engines of this process:
  * 0 = mma.sync, 1 = wgmma one 128 x 128 tile per CTA, 2 (default) = persistent 128 x 256 wgmma kernel,
  * -1 = query only; returns the current setting. Bits 8..11 of a
